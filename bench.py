@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- body-steps/sec of the Edyn per-step hot path on B200 (BASELINE.json metric).
+"""bench.py -- body-steps/sec of the Edyn per-step hot path on H100 (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b2d|reference] [--workload NAME]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b2d|reference] [--workload NAME] [--dump-outputs DIR]
 
 A "step" is one fixed simulation step (broadphase -> narrowphase -> islands -> solve -> integrate) of the whole scene.
 
@@ -20,9 +20,10 @@ Workload (same at every N, so the driver's 1 -> 8 comparison is a STRONG-scaling
 Keys beyond the base contract:
   roofline      velocity-solve kernel: algorithmic bytes (388 B per contact point per velocity iteration, 544 B per hinge
                 per iteration, + 0.75 pass for the warm start; SURVEY.md section 8d) / mean CUDA-event duration of that
-                kernel over the timed steps, against MEASURED_PEAKS.json's HBM copy bandwidth.
+                kernel over the timed steps, against MEASURED_PEAKS.json's HBM copy bandwidth where that file exists, else
+                the H100 SXM data sheet's 3.35 TB/s.
   cpu_baseline  rank 0, N = 1 only.  kind "reference": the reference's OWN stepper (oracle/_ref/libedyn_stepper.so =
-                /root/reference/src/edyn compiled unmodified against oracle/entt_lite), execution_mode
+                the reference's src/edyn compiled unmodified against oracle/entt_lite), execution_mode
                 sequential_multithreaded on all host threads, on a bounded SLICE of the workload (same generator, fewer
                 chains / a smaller pile: REF_SLICE) -- the full chain scene cannot be run by the reference in bounded
                 time (entity_graph::insert_edge walks the plane's adjacency list for every new contact: quadratic in the
@@ -31,6 +32,9 @@ Keys beyond the base contract:
                 Where the stepper library is absent the port is the cpu_baseline (kind "port").
   e2e           same metric through the C ABI with HOST buffers: every step uploads the body state from pinned
                 host memory (b2d_upload_state), steps, and downloads it again (b2d_download_state).
+  --dump-outputs DIR  N = 1: after the timed steps, the body state the timed path computed in its last step (what
+                b2d_download_state hands a caller: pos, orn, linvel, angvel of every body of the top workload, float32) as
+                DIR/<name>.npy.  The scenes are generated from fixed seeds, so the same arguments give the same inputs.
 --impl reference times the reference's CPU path: the real stepper on the slice above when oracle/_ref holds it (the line
 also carries `port`, the oracle port on the full workload), else the oracle port on the full workload.
 """
@@ -82,11 +86,11 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks + throttle reasons during the timed region."""
     Q = "clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -257,7 +261,7 @@ def reference_real(args, name, steps, warmup, settle, budget_s):
     dt = time.perf_counter() - t0
     value = scene["dynamic"] * steps / dt
     sample = f"{scene['name']}: {scene['dynamic']} of the workload's dynamic bodies (same generator and settings), the reference's own " \
-             f"stepper_sequential compiled from /root/reference against oracle/entt_lite, execution_mode sequential_multithreaded with " \
+             f"stepper_sequential compiled from the reference's sources against oracle/entt_lite, execution_mode sequential_multithreaded with " \
              f"{threads} workers{calib}, {n_settle} untimed settle steps, {steps} timed steps"
     return scene, value, dt, sample, threads
 
@@ -328,20 +332,26 @@ def solver_roofline(st, scene, step_ms):
             "integrate": {"kernel": "k_integrate", "achieved": integ_gbs, "frac": integ_gbs / peak, "kernel_ms": st["integrate_ms"]}}
 
 
-def traffic_for(name):
-    """dram__bytes_read.sum + dram__bytes_write.sum of the solve kernel per launch from the committed ncu capture."""
-    for fn in ("traffic_r02.json", "traffic_r01.json"):
-        p = os.path.join(ROOT, "profiles", fn)
-        if os.path.exists(p):
-            tj = json.load(open(p))
-            ent = tj.get(name) if isinstance(tj.get(name), dict) else (tj if tj.get("workload") == name else None)
-            if ent and "k_solve" in ent:
-                return ent["k_solve"]["dram_bytes_read"] + ent["k_solve"]["dram_bytes_write"]
-    return None
+DUMP_LIMIT_BYTES = 64 << 20
 
 
-def measure_single(args, name, local_rank, steps, warmup, cpu_seconds, sample_clocks, real_reference=False):
-    """One workload, whole scene on one GPU: device-resident value, e2e through host buffers, roofline, CPU baseline."""
+def dump_outputs(out_dir, state):
+    """The arrays of one download_state, one .npy file each (float32).  A state larger than DUMP_LIMIT_BYTES is cut to a
+    fixed, seeded sample of bodies; body_index.npy (float64) then says which."""
+    os.makedirs(out_dir, exist_ok=True)
+    n = len(state["pos"])
+    row_bytes = sum(v.nbytes // max(n, 1) for v in state.values())
+    if n * row_bytes > DUMP_LIMIT_BYTES:
+        keep = np.sort(np.random.default_rng(0).choice(n, size=(DUMP_LIMIT_BYTES - (1 << 20)) // (row_bytes + 8), replace=False))
+        state = {k: v[keep] for k, v in state.items()}
+        np.save(os.path.join(out_dir, "body_index.npy"), keep.astype(np.float64))
+    for k, v in state.items():
+        np.save(os.path.join(out_dir, f"{k}.npy"), np.ascontiguousarray(v, np.float32))
+
+
+def measure_single(args, name, local_rank, steps, warmup, cpu_seconds, sample_clocks, real_reference=False, dump_dir=None):
+    """One workload, whole scene on one GPU: device-resident value, e2e through host buffers, roofline, CPU baseline.
+    dump_dir: where the state after the last timed step goes (dump_outputs)."""
     import torch
     import edyn_b200 as E
     scene = make_scene(name, args.scale)
@@ -371,6 +381,8 @@ def measure_single(args, name, local_rank, steps, warmup, cpu_seconds, sample_cl
     st = w.stats()
     launches = st["kernel_launches"] - launches0 - 1        # minus the stats kernel itself
     value = n_dyn * steps / (ms * 1e-3)
+    if dump_dir:
+        dump_outputs(dump_dir, w.download_state(aabb=False))
 
     # ---- end to end through the C ABI with host buffers
     n_all = w.num_bodies
@@ -397,7 +409,6 @@ def measure_single(args, name, local_rank, steps, warmup, cpu_seconds, sample_cl
     bytes_state = n_all * 13 * 4
 
     roofline = solver_roofline(st, scene, ms / steps)
-    roofline["traffic"] = traffic_for(name) if args.scale == 1.0 else None
 
     cpu = None
     if cpu_seconds > 0:
@@ -425,7 +436,7 @@ def measure_single(args, name, local_rank, steps, warmup, cpu_seconds, sample_cl
                       "velocity_iterations": scene["settings"]["velocity_iterations"], "position_iterations": scene["settings"]["position_iterations"],
                       "settle_steps": SETTLE_STEPS, "manifolds": st["manifolds"], "contact_points": st["contact_points"], "hinges": st["hinges"],
                       "contact_colors": st["contact_colors"], "islands": st["islands"],
-                      "l2": "inputs change every step and the per-step working set (rows + manifolds + bodies) exceeds the 126 MB L2 for the "
+                      "l2": "inputs change every step and the per-step working set (rows + manifolds + bodies) exceeds the 50 MB L2 for the "
                             "two large configs; no explicit flush"},
            "gpu_launches": int(launches),
            "e2e": {"value": e2e_value, "unit": "body-steps/s", "h2d_bytes_per_step": bytes_state, "d2h_bytes_per_step": bytes_state, "steps": e2e_steps},
@@ -441,7 +452,8 @@ def measure_single(args, name, local_rank, steps, warmup, cpu_seconds, sample_cl
 
 
 def run_single(args, local_rank):
-    top = measure_single(args, args.workload, local_rank, args.steps, args.warmup, 0 if args.no_cpu else args.cpu_seconds, True, real_reference=True)
+    top = measure_single(args, args.workload, local_rank, args.steps, args.warmup, 0 if args.no_cpu else args.cpu_seconds, True, real_reference=True,
+                         dump_dir=args.dump_outputs)
     line = {"metric": "body-steps/sec", "value": top["value"], "unit": "body-steps/s", "n_gpus": 1, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": top["ms_per_step"], "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
             "config": dict(top["config"], parallelism="1 GPU: whole scene in one device world"),
@@ -609,6 +621,8 @@ def run_device(args):
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     if world_size > 1:
+        if args.dump_outputs:
+            raise SystemExit("--dump-outputs is only supported with one GPU")
         run_sharded(args, world_size, rank, local_rank)
     else:
         torch.cuda.set_device(local_rank)
@@ -630,6 +644,8 @@ def main():
     ap.add_argument("--ref-real-seconds", type=float, default=75.0, help="device arm: budget of the real reference stepper's cpu_baseline leg")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--ref-child", default=None, help=argparse.SUPPRESS)
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="N = 1: write the body state after the last timed step as DIR/<name>.npy (float32)")
     ap.add_argument("--exact-exchange", action="store_true", help="N > 1: read every step's rank boxes before the next step starts (no look-ahead margin)")
     args = ap.parse_args()
     if args.ref_child:

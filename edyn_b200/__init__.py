@@ -1,6 +1,6 @@
-"""edyn_b200 -- B200-native replacement for Edyn's per-step rigid-body hot path.
+"""edyn_b200 -- H100-native replacement for Edyn's per-step rigid-body hot path.
 
-Host adapter (this package) -> C ABI (include/b2d.h, edyn_b200/libb2d.so) -> hand-written sm_100a kernels
+Host adapter (this package) -> C ABI (include/b2d.h, edyn_b200/libb2d.so) -> hand-written sm_90a kernels
 (edyn_b200/csrc).  See DESIGN.md.  Importing this package never imports oracle/.
 """
 from ._lib import B2DError, build  # noqa: F401

@@ -7,7 +7,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("B2D_LIB") or os.path.join(HERE, "libb2d.so")     # B2D_LIB: development builds
 SRC = os.path.join(HERE, "csrc", "b2d_api.cu")
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-fmad=false",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-fmad=false",
               "-Xcompiler", "-fPIC", "-shared"]
 
 
@@ -16,7 +16,7 @@ class B2DError(RuntimeError):
 
 
 def build(force=False):
-    """nvcc cross-compiles the whole CUDA path for sm_100a into edyn_b200/libb2d.so (in-tree)."""
+    """nvcc cross-compiles the whole CUDA path for sm_90a into edyn_b200/libb2d.so (in-tree)."""
     srcs = [os.path.join(HERE, "csrc", f) for f in os.listdir(os.path.join(HERE, "csrc")) if f.endswith((".cu", ".cuh"))]
     srcs.append(os.path.join(HERE, "..", "include", "b2d.h"))
     if not force and os.path.exists(LIB_PATH) and all(os.path.getmtime(s) <= os.path.getmtime(LIB_PATH) for s in srcs):

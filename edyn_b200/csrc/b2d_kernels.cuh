@@ -1,4 +1,4 @@
-// CUDA kernels of the per-step hot path (sm_100a).  One section per reference phase:
+// CUDA kernels of the per-step hot path (sm_90a).  One section per reference phase:
 //   broadphase   src/edyn/collision/broadphase.cpp:119-195      -> k_bp_*
 //   narrowphase  src/edyn/collision/narrowphase.cpp:21-40        -> k_narrowphase
 //   islands      src/edyn/simulation/island_manager.cpp:117-247  -> k_cc_*

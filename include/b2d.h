@@ -1,5 +1,5 @@
 /*
- * b2d.h -- C ABI of the B200-native Edyn step ("b2d" = B200 dynamics).
+ * b2d.h -- C ABI of the GPU-native Edyn step ("b2d": the project's original name).
  *
  * Drop-in boundary (SURVEY.md section 8b, DESIGN.md section 2).  The reference has no FFI; its boundary is
  * four C++ objects called in fixed order from

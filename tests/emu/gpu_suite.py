@@ -1,11 +1,11 @@
 """TEST INFRASTRUCTURE / development aid.  Runs the `-m gpu` tests that do not need torch's CUDA tensors against the CPU
-emulation (tests/emu) instead of a B200: the kernels' logic, the C ABI, the Python adapter, the C++ EnTT binding.
+emulation (tests/emu) instead of a GPU: the kernels' logic, the C ABI, the Python adapter, the C++ EnTT binding.
 
     python tests/emu/gpu_suite.py [extra pytest args]
 
 Not run: the full-size configs and the 1000-step box stack (hours under emulation), the hand-over tests (their payloads live
 in torch CUDA tensors), the NCCL tests, the C++ adapter's hello_world (links libb2d.so by name).
-State at the end of round 2: 32 tests, all green (the same tests were green on a B200 before the last kernel clean-up;
+State at the end of round 2: 32 tests, all green (the same tests were green on a GPU before the last kernel clean-up;
 tests/test_zz_gpu_stepper_b2d.py has only ever run here)."""
 import os
 import subprocess

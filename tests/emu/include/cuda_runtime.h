@@ -155,7 +155,7 @@ inline const char *cudaGetErrorString(cudaError_t e) { return e == cudaSuccess ?
 inline cudaError_t cudaGetLastError() { return cudaSuccess; }
 inline cudaError_t cudaGetDeviceCount(int *n) { *n = 1; return cudaSuccess; }
 inline cudaError_t cudaSetDevice(int) { return cudaSuccess; }
-inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp *p, int) { std::memset(p, 0, sizeof(*p)); std::strcpy(p->name, "CPU emulation (tests/emu)"); p->multiProcessorCount = 2; p->cooperativeLaunch = 1; p->major = 10; return cudaSuccess; }
+inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp *p, int) { std::memset(p, 0, sizeof(*p)); std::strcpy(p->name, "CPU emulation (tests/emu)"); p->multiProcessorCount = 2; p->cooperativeLaunch = 1; p->major = 9; return cudaSuccess; }
 template<typename T> inline cudaError_t cudaMalloc(T **p, size_t bytes) { *p = static_cast<T *>(std::aligned_alloc(256, (bytes + 255) / 256 * 256 + 256)); return *p ? cudaSuccess : cudaErrorMemoryAllocation; }
 inline cudaError_t cudaFree(void *p) { std::free(p); return cudaSuccess; }
 inline cudaError_t cudaMemcpy(void *d, const void *s, size_t n, cudaMemcpyKind) { std::memmove(d, s, n); return cudaSuccess; }

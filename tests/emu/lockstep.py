@@ -1,5 +1,5 @@
 """TEST INFRASTRUCTURE.  The library's CUDA kernels, executed by the CPU emulation (tests/emu), in lock step with the
-oracle through the normal Python adapter and C ABI -- the same comparison tests/test_gpu_parity.py makes on a B200: ordered
+oracle through the normal Python adapter and C ABI -- the same comparison tests/test_gpu_parity.py makes on the GPU: ordered
 pair lists identical, post-solve state within 1e-5 (here: identical, glibc's sinf / cosf on both sides) with the oracle
 replaying the device's Gauss-Seidel order, manifolds and joint impulses re-synchronised every step.
 
@@ -122,19 +122,17 @@ def lockstep_with_mutations(E, O, scene, steps, seed):
 def free_run_against_real_stepper(E, O):
     """No oracle in between: the kernels (emulated) and the reference's real stepper, both free-running from the same scene.
     Hinge chains are insensitive to the sweep order (tiny islands at rest), so the two must simply agree; hello_world must be
-    identical while the box falls."""
+    identical while the box falls.  The reference's side is its recorded states (tests/golden/free_run.npz)."""
     import numpy as np
     from tests.golden import make_whole_step as G
     out = []
-    for name, scene, marks in (("chains_64", E.scenes.hinge_chains(4, 4), (60, 300)), ("hello_world", E.scenes.hello_world(), (24,))):
-        st = scene["settings"]
+    for name in ("chains_64", "hello_world"):
+        scene, marks = G.free_run_scene(E, name), G.FREE_RUN[name][2]
         w = E.scenes.build_world(scene)
-        r = O.RefWorld(vel_iters=st["velocity_iterations"], pos_iters=st["position_iterations"])
-        G.populate(r, scene)
         n, done = scene["dynamic"], 0
         for m in marks:
-            w.step(m - done); r.step(m - done); done = m
-            g, c = w.download_state(), r.state()
+            w.step(m - done); done = m
+            g, c = w.download_state(), G.reference_free_run(name, m)
             out.append(dict(scene=name, step=m, dpos=float(np.abs(g["pos"][:n] - c["pos"][:n]).max()), dvel=float(np.abs(g["linvel"][:n] - c["linvel"][:n]).max())))
         w.close()
     return out

@@ -6,7 +6,9 @@ island.edges; that order is EnTT pool order after entity_graph traversals, so it
 
     python tests/golden/make_whole_step.py          # needs /root/reference at build time; the .npz travels, the reference does not
 
-Consumer: tests/test_ref_stepper.py::test_oracle_replays_reference_trajectories (CPU, runs without the library)."""
+Consumer: tests/test_ref_stepper.py::test_oracle_replays_reference_trajectories (CPU, runs without the library).
+It also writes tests/golden/free_run.npz, the reference's free-running end states that the device (and its CPU emulation)
+is compared with: tests/test_zz_gpu_stepper_b2d.py, tests/test_emu_device.py."""
 import os
 import sys
 
@@ -26,6 +28,24 @@ SCENES = {
     "chains_16": ("hinge_chains", (2, 2)),
 }
 SCENE_KW = {"mixed_125": {"jitter": 0.01}}
+# free_run.npz: the reference's state, nothing replayed, after the listed step counts.  name -> (factory, args, steps)
+FREE_RUN = {
+    "chains_64": ("hinge_chains", (4, 4), (60, 300)),
+    "hello_world": ("hello_world", (), (24,)),
+    "chains_256": ("hinge_chains", (8, 8), (1000,)),
+}
+FREE_RUN_PATH = os.path.join(ROOT, "tests", "golden", "free_run.npz")
+
+
+def free_run_scene(E, name):
+    fn, a, _ = FREE_RUN[name]
+    return getattr(E.scenes, fn)(*a)
+
+
+def reference_free_run(name, step):
+    """pos and linvel of the scene's dynamic bodies after `step` free-running steps of the reference's own stepper."""
+    g = np.load(FREE_RUN_PATH)
+    return {k: g[f"{name}.{step}.{k}"] for k in ("pos", "linvel")}
 
 
 def build_scene(E, name):
@@ -75,6 +95,22 @@ def main():
               f"{int(c['num'].sum())} points at the end")
     out["steps"] = np.asarray([STEPS, KEEP_EVERY], np.uint32)
     np.savez_compressed(os.path.join(ROOT, "tests", "golden", "whole_step.npz"), **out)
+    write_free_run(E, O)
+
+
+def write_free_run(E, O):
+    free = {}
+    for name, (_, _, marks) in FREE_RUN.items():
+        scene = free_run_scene(E, name)
+        st = scene["settings"]
+        r = O.RefWorld(vel_iters=st["velocity_iterations"], pos_iters=st["position_iterations"])
+        populate(r, scene)
+        n, done = scene["dynamic"], 0
+        for m in marks:
+            r.step(m - done); done = m
+            x = r.state()
+            free[f"{name}.{m}.pos"], free[f"{name}.{m}.linvel"] = x["pos"][:n].copy(), x["linvel"][:n].copy()
+    np.savez_compressed(FREE_RUN_PATH, **free)
 
 
 if __name__ == "__main__":

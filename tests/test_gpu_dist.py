@@ -106,7 +106,7 @@ def test_island_migration_two_gpus(gpu, E):
     world tracks a single-GPU run of the whole scene."""
     import torch
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs two GPUs (run under gpurun --gpus 2)")
+        pytest.skip("needs two GPUs")
     import torch.multiprocessing as mp
     ctx = mp.get_context("spawn")
     q = ctx.Queue()

@@ -336,7 +336,7 @@ def test_handover_two_gpus_nccl(gpu, E, scene_name, steps):
     """The same hand-over with one process per GPU and the blobs travelling as device buffers over NCCL send / recv."""
     import torch
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs two GPUs (gpurun --gpus 2); the threaded flavour above covers the library path on one")
+        pytest.skip("needs two GPUs; the threaded flavour above covers the library path on one")
     import torch.multiprocessing as mp
     ctx = mp.get_context("spawn")
     q = ctx.Queue()

@@ -87,29 +87,23 @@ def test_device_binding_follows_the_real_cpu_stepper(dev, E, O):
 
 
 def test_device_chains_follow_the_real_stepper_free_running(gpu, E, O):
-    """No oracle in between: the B200 and the reference's real stepper_sequential, both free-running for 1000 steps on a
+    """No oracle in between: the device and the reference's real stepper_sequential, both free-running for 1000 steps on a
     slice of config 5 (64 chains): the hinge-chain family is insensitive to the sweep order, so north_star's 1e-4 must
-    simply hold (5e-10 absolute under the CPU emulation of the kernels after 300 steps)."""
-    if O.ref_stepper() is None:
-        pytest.skip("oracle/_ref/libedyn_stepper.so not shipped")
-    scene = E.scenes.hinge_chains(8, 8)
-    st = scene["settings"]
+    simply hold (5e-10 absolute under the CPU emulation of the kernels after 300 steps).  The reference's side is its
+    recorded end state (tests/golden/free_run.npz)."""
+    scene = G.free_run_scene(E, "chains_256")
     w = E.scenes.build_world(scene)
-    r = O.RefWorld(vel_iters=st["velocity_iterations"], pos_iters=st["position_iterations"])
-    G.populate(r, scene)
     n = scene["dynamic"]
-    w.step(1000); r.step(1000)
-    g, c = w.download_state(aabb=False), r.state()
+    w.step(1000)
+    g, c = w.download_state(aabb=False), G.reference_free_run("chains_256", 1000)
     rel = float(np.abs(g["pos"][:n] - c["pos"][:n]).max() / np.abs(c["pos"][:n]).max())
     assert rel <= 1e-4, f"relative position error after 1000 steps {rel:.3e}"
     assert float(np.abs(g["linvel"][:n] - c["linvel"][:n]).max()) <= 1e-3
     w.close()
 
 
-@pytest.mark.xfail(strict=False, reason="first run on hardware: the restitution solver was written after the round's GPU budget ended and is "
-                                        "verified under the CPU emulation only (tests/test_emu_device.py::test_emulated_restitution_solver)")
 def test_device_restitution_solver_matches_oracle(gpu, E, O):
-    """B2D_FLAG_RESTITUTION_SOLVER on the B200 in lock step with the oracle's restatement of restitution_solver.cpp (the
+    """B2D_FLAG_RESTITUTION_SOLVER on the device in lock step with the oracle's restatement of restitution_solver.cpp (the
     reference's default settings), mixed pile with e = 0.2 and a random scene with e up to 0.8."""
     from tests.emu.lockstep import lockstep
     from tests.test_ref_stepper import random_scene
