@@ -631,8 +631,9 @@ static int enqueue_solver_a(b2d_world *w, int recolor) {
     CK(cub::DeviceRadixSort::SortPairs(w->cub_tmp, t, d.hkey, d.hkey_s, d.hidx, d.hidx_s, (int)d.NH, 0, COLOR_KEY_BITS, s)); w->launches += 3;
     LAUNCH(k_color_offsets, d.NM, 256, d);
     LAUNCH(k_color_fixup, 1, 32, d);
-    LAUNCH(k_prepare_contacts, d.NM, 256, d);
-    if (d.nhinges) LAUNCH(k_prepare_hinges, d.nhinges, 256, d);
+    const int fused = (d.max_tiles && w->cfg.position_iterations > 0) ? 1 : 0;        // k_island_tiles prepares the tiled rows
+    LAUNCH(k_prepare_contacts, d.NM, 256, d, fused);
+    if (d.nhinges) LAUNCH(k_prepare_hinges, d.nhinges, 256, d, fused);
     return B2D_OK;
 }
 static int enqueue_solver_b(b2d_world *w) {
@@ -988,11 +989,13 @@ int b2d_download_solver_order(b2d_world *w, uint32_t *hinge_ids, uint32_t *nh, u
     Counters c; int rc = fetch_counters(w, c); if (rc) return rc;
     const uint32_t na = c.nactive, nhh = c.nhactive;
     if (na > *nm || nhh > *nh) { w->error = "b2d_download_solver_order: capacity too small"; return B2D_ERR_CAPACITY; }
-    std::vector<uint4> hdr(na), hh(nhh);
-    std::vector<uint32_t> ck(na), hk(nhh);
-    if (na) CK(cudaMemcpyAsync(hdr.data(), w->d.hdr, na * sizeof(uint4), cudaMemcpyDeviceToHost, w->stream));
+    // the row headers (hdr / hhdr) are not written for tiled constraints: the pairs come from the manifolds themselves
+    std::vector<uint2> mp(na ? w->d.NM : 0);
+    std::vector<uint32_t> ck(na), hk(nhh), ci(na), hi(nhh);
+    if (na) CK(cudaMemcpyAsync(mp.data(), w->d.mpair, w->d.NM * sizeof(uint2), cudaMemcpyDeviceToHost, w->stream));
+    if (na) CK(cudaMemcpyAsync(ci.data(), w->d.cidx_s, na * sizeof(uint32_t), cudaMemcpyDeviceToHost, w->stream));
     if (na) CK(cudaMemcpyAsync(ck.data(), w->d.ckey_s, na * sizeof(uint32_t), cudaMemcpyDeviceToHost, w->stream));
-    if (nhh) CK(cudaMemcpyAsync(hh.data(), w->d.hhdr, nhh * sizeof(uint4), cudaMemcpyDeviceToHost, w->stream));
+    if (nhh) CK(cudaMemcpyAsync(hi.data(), w->d.hidx_s, nhh * sizeof(uint32_t), cudaMemcpyDeviceToHost, w->stream));
     if (nhh) CK(cudaMemcpyAsync(hk.data(), w->d.hkey_s, nhh * sizeof(uint32_t), cudaMemcpyDeviceToHost, w->stream));
     CK(cudaStreamSynchronize(w->stream));
     // The device arrays are tile-major for the tiled islands; the serial sweep that reproduces the per-body order is
@@ -1003,8 +1006,8 @@ int b2d_download_solver_order(b2d_world *w, uint32_t *hinge_ids, uint32_t *nh, u
     auto colour = [](uint32_t key) { return (key & KEY_DF) ? (key >> KEY_DF_COLOR_SHIFT) & 63u : key & 63u; };
     std::stable_sort(oc.begin(), oc.end(), [&](uint32_t x, uint32_t y) { return colour(ck[x]) < colour(ck[y]); });
     std::stable_sort(oh.begin(), oh.end(), [&](uint32_t x, uint32_t y) { return colour(hk[x]) < colour(hk[y]); });
-    for (uint32_t i = 0; i < na; ++i) { pairs[2 * i] = hdr[oc[i]].x & 0x7FFFFFFFu; pairs[2 * i + 1] = hdr[oc[i]].y & 0x7FFFFFFFu; }
-    for (uint32_t i = 0; i < nhh; ++i) hinge_ids[i] = hh[oh[i]].z;
+    for (uint32_t i = 0; i < na; ++i) { const uint2 p = mp[ci[oc[i]]]; pairs[2 * i] = p.x; pairs[2 * i + 1] = p.y; }
+    for (uint32_t i = 0; i < nhh; ++i) hinge_ids[i] = hi[oh[i]];
     *nm = na; *nh = nhh;
     return B2D_OK;
 }

@@ -1020,12 +1020,67 @@ B2D_D float rel_speed(v3 J0, v3 J1, v3 J2, v3 J3, v3 vA, v3 wA, v3 vB, v3 wB) {
     return dot(J0, vA) + dot(J1, wA) + dot(J2, vB) + dot(J3, wB);
 }
 
-// contact_constraint::prepare (contact_constraint.cpp:15-56) + prepare_row per sorted manifold; rows are
-// written in colour order so the solve kernel streams them.  Row storage keeps (n, rA, rB) and rebuilds the
-// Jacobian in registers: 84 B/point instead of the reference's 312 B (constraint_row + _friction).
-__global__ void __launch_bounds__(256) k_prepare_contacts(Dev d) {
-    const uint32_t n = d.cnt->nactive;
-    GRID_STRIDE(i, n) {
+// contact_constraint::prepare (contact_constraint.cpp:15-56) + prepare_row of contact point slot mi: r0 = normal | rhs,
+// r1 = rA | eff_mass, r2 = rB | friction, r3 = eff_mass t0, t1, rhs t0, t1, im = warm-start impulses (n, t0, t1).
+// Row storage keeps (n, rA, rB) and rebuilds the Jacobian in registers: 84 B/point instead of the reference's 312 B
+// (constraint_row + _friction).  Shared by k_prepare_contacts and k_island_tiles, so both produce the same bits.
+B2D_D void contact_point_rows(const Dev &d, size_t mi, const SBody &A, const SBody &B, v3 posA, q4 ornA, v3 posB, q4 ornB,
+                              float4 &r0, float4 &r1, float4 &r2, float4 &r3, float4 &imp) {
+    float4 a4 = d.pA[mi], b4 = d.pB[mi], n4 = d.pN[mi], im = d.pI[mi];
+    v3 normal = mk3(n4);
+    v3 pAw = to_world(mk3(a4), posA, ornA), pBw = to_world(mk3(b4), posB, ornB);
+    v3 rA = pAw - posA, rB = pBw - posB;
+    v3 J1 = cross(rA, normal), J2 = -normal, J3 = -cross(rB, normal);
+    float em = eff_mass(normal, J1, J2, J3, A, B);
+    float error = 0.0f;
+    if (a4.w > 0) error = a4.w / d.dt;
+    float relvel = rel_speed(normal, J1, J2, J3, A.v, A.w, B.v, B.w);
+    float rhs = -(error * 0.2f + relvel * (1.0f + (d.rest_iters ? 0.0f : n4.w)));     // solver.cpp:217-236
+    v3 t, u; plane_space(normal, t, u);
+    v3 T1 = cross(rA, t), T2 = -t, T3 = -cross(rB, t);
+    v3 U1 = cross(rA, u), U2 = -u, U3 = -cross(rB, u);
+    float em_t = eff_mass(t, T1, T2, T3, A, B), em_u = eff_mass(u, U1, U2, U3, A, B);
+    float rhs_t = -rel_speed(t, T1, T2, T3, A.v, A.w, B.v, B.w), rhs_u = -rel_speed(u, U1, U2, U3, A.v, A.w, B.v, B.w);
+    r0 = f4(normal, rhs); r1 = f4(rA, em); r2 = f4(rB, b4.w);
+    r3 = make_float4(em_t, em_u, rhs_t, rhs_u);
+    imp = make_float4(im.x, im.y, im.z, 0);
+}
+
+// hinge_constraint::prepare, hinge_constraint.cpp:26-69 (no limits / springs / torque rows): the 7 row vectors of hinge h
+// (rA | em0, rB | em1, p | em2, q | em3, em4 rhs0 rhs1 rhs2, rhs3 rhs4 imp0 imp1, imp2 imp3 imp4) to R[0], R[stride], ...
+// Shared by k_prepare_hinges and k_island_tiles.
+B2D_D void hinge_rows(const Dev &d, uint32_t h, const SBody &A, const SBody &B, v3 posA, q4 ornA, v3 posB, q4 ornB,
+                      float4 *R, uint32_t stride) {
+    v3 rA = to_world(mk3(d.hpivA[h]), posA, ornA) - posA;
+    v3 rB = to_world(mk3(d.hpivB[h]), posB, ornB) - posB;
+    v3 p = rotate(ornA, mk3(d.hfA1[h])), q = rotate(ornA, mk3(d.hfA2[h]));
+    float em[5], rhs[5];
+    #pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        v3 e = axis_vec(k);
+        // rows of skew(r): (0,-z,y), (z,0,-x), (-y,x,0)  matrix3x3.hpp:243-249
+        v3 sa = k == 0 ? mk3(0, -rA.z, rA.y) : (k == 1 ? mk3(rA.z, 0, -rA.x) : mk3(-rA.y, rA.x, 0));
+        v3 sb = k == 0 ? mk3(0, -rB.z, rB.y) : (k == 1 ? mk3(rB.z, 0, -rB.x) : mk3(-rB.y, rB.x, 0));
+        v3 J1 = -sa, J2 = -e, J3 = sb;
+        em[k] = eff_mass(e, J1, J2, J3, A, B);
+        rhs[k] = -(0.0f * 0.2f + rel_speed(e, J1, J2, J3, A.v, A.w, B.v, B.w) * (1.0f + 0.0f));
+    }
+    const v3 z = mk3(0, 0, 0);
+    em[3] = eff_mass(z, p, z, -p, A, B); rhs[3] = -(0.0f * 0.2f + rel_speed(z, p, z, -p, A.v, A.w, B.v, B.w) * (1.0f + 0.0f));
+    em[4] = eff_mass(z, q, z, -q, A, B); rhs[4] = -(0.0f * 0.2f + rel_speed(z, q, z, -q, A.v, A.w, B.v, B.w) * (1.0f + 0.0f));
+    const float *imp = d.himp + 5 * (size_t)h;
+    R[0] = f4(rA, em[0]); R[stride] = f4(rB, em[1]); R[2 * stride] = f4(p, em[2]); R[3 * stride] = f4(q, em[3]);
+    R[4 * stride] = make_float4(em[4], rhs[0], rhs[1], rhs[2]);
+    R[5 * stride] = make_float4(rhs[3], rhs[4], imp[0], imp[1]);
+    R[6 * stride] = make_float4(imp[2], imp[3], imp[4], 0);
+}
+
+// Row preparation per sorted manifold; rows are written in colour order so the solve kernel streams them.  With fused
+// != 0 k_island_tiles prepares the tiled range [0, ntiled) itself and this kernel starts after it.
+__global__ void __launch_bounds__(256) k_prepare_contacts(Dev d, int fused) {
+    const uint32_t n = d.cnt->nactive, first = fused ? d.cnt->ntiled : 0u;
+    GRID_STRIDE(j, n - first) {
+        const uint32_t i = first + j;
         uint32_t m = d.cidx_s[i];
         uint2 pr = d.mpair[m];
         uint32_t npts = d.mstate[m] & MS_NPTS_MASK;
@@ -1051,62 +1106,26 @@ __global__ void __launch_bounds__(256) k_prepare_contacts(Dev d) {
             { const uint32_t l = d.parent[pr.x]; d.pisl[i] = l != 0xFFFFFFFFu ? l : d.parent[pr.y]; }
         }
         for (uint32_t s = 0; s < npts; ++s) {
-            size_t mi = (size_t)s * d.NM + m, ri = (size_t)s * d.NM + i;
-            float4 a4 = d.pA[mi], b4 = d.pB[mi], n4 = d.pN[mi], im = d.pI[mi];
-            v3 normal = mk3(n4);
-            v3 pAw = to_world(mk3(a4), posA, ornA), pBw = to_world(mk3(b4), posB, ornB);
-            v3 rA = pAw - posA, rB = pBw - posB;
-            v3 J1 = cross(rA, normal), J2 = -normal, J3 = -cross(rB, normal);
-            float em = eff_mass(normal, J1, J2, J3, A, B);
-            float error = 0.0f;
-            if (a4.w > 0) error = a4.w / d.dt;
-            float relvel = rel_speed(normal, J1, J2, J3, A.v, A.w, B.v, B.w);
-            float rhs = -(error * 0.2f + relvel * (1.0f + (d.rest_iters ? 0.0f : n4.w)));     // solver.cpp:217-236
-            v3 t, u; plane_space(normal, t, u);
-            v3 T1 = cross(rA, t), T2 = -t, T3 = -cross(rB, t);
-            v3 U1 = cross(rA, u), U2 = -u, U3 = -cross(rB, u);
-            float em_t = eff_mass(t, T1, T2, T3, A, B), em_u = eff_mass(u, U1, U2, U3, A, B);
-            float rhs_t = -rel_speed(t, T1, T2, T3, A.v, A.w, B.v, B.w), rhs_u = -rel_speed(u, U1, U2, U3, A.v, A.w, B.v, B.w);
-            d.R0[ri] = f4(normal, rhs); d.R1[ri] = f4(rA, em); d.R2[ri] = f4(rB, b4.w);
-            d.R3[ri] = make_float4(em_t, em_u, rhs_t, rhs_u);
-            d.IMP[ri] = make_float4(im.x, im.y, im.z, 0);
+            const size_t ri = (size_t)s * d.NM + i;
+            float4 r0, r1, r2, r3, im;
+            contact_point_rows(d, (size_t)s * d.NM + m, A, B, posA, ornA, posB, ornB, r0, r1, r2, r3, im);
+            d.R0[ri] = r0; d.R1[ri] = r1; d.R2[ri] = r2; d.R3[ri] = r3; d.IMP[ri] = im;
         }
     }
 }
 
-// hinge_constraint::prepare, hinge_constraint.cpp:26-69 (no limits / springs / torque rows)
-__global__ void k_prepare_hinges(Dev d) {
-    const uint32_t n = d.cnt->nhactive;
-    GRID_STRIDE(i, n) {
+// per sorted hinge; fused as in k_prepare_contacts ([0, nhtiled) is prepared by k_island_tiles)
+__global__ void k_prepare_hinges(Dev d, int fused) {
+    const uint32_t n = d.cnt->nhactive, first = fused ? d.cnt->nhtiled : 0u;
+    GRID_STRIDE(j, n - first) {
+        const uint32_t i = first + j;
         uint32_t h = d.hidx_s[i];
         uint2 pr = d.hpair[h];
         uint32_t fa = d.flags[pr.x], fb = d.flags[pr.y];
         SBody A = solver_body(d, pr.x, fa), B = solver_body(d, pr.y, fb);
         v3 posA = mk3(d.pos[pr.x]), posB = mk3(d.pos[pr.y]);
         q4 ornA = mkq(d.orn[pr.x]), ornB = mkq(d.orn[pr.y]);
-        v3 rA = to_world(mk3(d.hpivA[h]), posA, ornA) - posA;
-        v3 rB = to_world(mk3(d.hpivB[h]), posB, ornB) - posB;
-        v3 p = rotate(ornA, mk3(d.hfA1[h])), q = rotate(ornA, mk3(d.hfA2[h]));
-        float em[5], rhs[5];
-        #pragma unroll
-        for (int k = 0; k < 3; ++k) {
-            v3 e = axis_vec(k);
-            // rows of skew(r): (0,-z,y), (z,0,-x), (-y,x,0)  matrix3x3.hpp:243-249
-            v3 sa = k == 0 ? mk3(0, -rA.z, rA.y) : (k == 1 ? mk3(rA.z, 0, -rA.x) : mk3(-rA.y, rA.x, 0));
-            v3 sb = k == 0 ? mk3(0, -rB.z, rB.y) : (k == 1 ? mk3(rB.z, 0, -rB.x) : mk3(-rB.y, rB.x, 0));
-            v3 J1 = -sa, J2 = -e, J3 = sb;
-            em[k] = eff_mass(e, J1, J2, J3, A, B);
-            rhs[k] = -(0.0f * 0.2f + rel_speed(e, J1, J2, J3, A.v, A.w, B.v, B.w) * (1.0f + 0.0f));
-        }
-        const v3 z = mk3(0, 0, 0);
-        em[3] = eff_mass(z, p, z, -p, A, B); rhs[3] = -(0.0f * 0.2f + rel_speed(z, p, z, -p, A.v, A.w, B.v, B.w) * (1.0f + 0.0f));
-        em[4] = eff_mass(z, q, z, -q, A, B); rhs[4] = -(0.0f * 0.2f + rel_speed(z, q, z, -q, A.v, A.w, B.v, B.w) * (1.0f + 0.0f));
-        const float *imp = d.himp + 5 * (size_t)h;
-        float4 *R = d.HR + 7 * (size_t)i;
-        R[0] = f4(rA, em[0]); R[1] = f4(rB, em[1]); R[2] = f4(p, em[2]); R[3] = f4(q, em[3]);
-        R[4] = make_float4(em[4], rhs[0], rhs[1], rhs[2]);
-        R[5] = make_float4(rhs[3], rhs[4], imp[0], imp[1]);
-        R[6] = make_float4(imp[2], imp[3], imp[4], 0);
+        hinge_rows(d, h, A, B, posA, ornA, posB, ornB, d.HR + 7 * (size_t)i, 1);
         d.hhdr[i] = make_uint4(pr.x | (A.proc ? 0u : 0x80000000u), pr.y | (B.proc ? 0u : 0x80000000u), h,
                                (A.proc ? d.bslot[pr.x] : SLOT_NONE) | ((B.proc ? d.bslot[pr.y] : SLOT_NONE) << 16));
         {
@@ -1655,15 +1674,28 @@ B2D_D uint32_t island_of(const Dev &d, uint32_t a, uint32_t b) { uint32_t l = d.
 // per-island max error of a tile, kept at the shared-memory slot of the island's root body
 B2D_D void tile_error_max(uint32_t *s_err, uint32_t islot, float err) { if (err != 0.0f) atomicMax(&s_err[islot], __float_as_uint(err)); }
 // ---------------------------------------------------------------------- island tiles: the whole solver.update on chip
-// velocity iterations + integrate_velocities + assign_applied_impulses + position iterations of the tiled islands in
-// ONE kernel: a tile's bodies, joints and manifolds are loaded once, the velocity iterations run, the bodies are integrated
+// row preparation + velocity iterations + integrate_velocities + assign_applied_impulses + position iterations of the
+// tiled islands in ONE kernel: a tile's bodies, joints and manifolds are loaded once and their rows computed on chip, the
+// velocity iterations run, the bodies are integrated
 // where they sit (shared memory), the impulses go straight to the warm-start cache, the position iterations run on
 // the same records, and positions / orientations / velocities are written once.  Same arithmetic in the same order as
-// the separate kernels (k_integrate, k_store_impulses skip what this kernel has done).
-// shared memory of a tile, float4 x TILE_CAP each: body records [0..7] -- velocity phase: dv, dw, inv_IW rows (| inv_m);
-// position phase: pos | inv_m, orn, inv_IW rows, inv_I rows --, joint rows [8..14], contact points 3-4 [15..24]
-// (solver rows, then pA pB pN pL)
+// the separate kernels (k_prepare_contacts, k_prepare_hinges, k_integrate, k_store_impulses skip what this kernel has done).
+// shared memory of a tile, float4 x TILE_CAP each: body records [0..7] -- row preparation: linvel, angvel, inv_IW rows
+// (| inv_m), pos, orn; velocity phase: dv, dw, inv_IW rows; position phase: pos | inv_m, orn, inv_IW rows, inv_I rows --,
+// joint rows [8..14], contact points 3-4 [15..24] (solver rows, then pA pB pN pL)
 constexpr size_t TILE_FUSED_SMEM = (8 + 7 + 10) * TILE_CAP * sizeof(float4);
+// solver_body (+ position, orientation, record slot) of body `id` of a tiled constraint during the row preparation: a
+// dynamic body from the records staged by slot, a static / kinematic one from global memory
+B2D_D void tile_solver_body(const Dev &d, const float4 *sb, uint32_t id, SBody &s, v3 &pos, q4 &orn, uint32_t &slot) {
+    const uint32_t f = d.flags[id];
+    if (!is_dynamic(f)) { s = solver_body(d, id, f); pos = mk3(d.pos[id]); orn = mkq(d.orn[id]); slot = SLOT_NONE; return; }
+    slot = d.bslot[id];
+    const float4 r0 = sb[2 * TILE_CAP + slot];
+    s.proc = true; s.inv_m = r0.w;
+    s.inv_I.r0 = mk3(r0); s.inv_I.r1 = mk3(sb[3 * TILE_CAP + slot]); s.inv_I.r2 = mk3(sb[4 * TILE_CAP + slot]);
+    s.v = mk3(sb[slot]); s.w = mk3(sb[TILE_CAP + slot]);
+    pos = mk3(sb[5 * TILE_CAP + slot]); orn = mkq(sb[6 * TILE_CAP + slot]);
+}
 B2D_D void tf_load(const float4 *sb, uint32_t tag, uint32_t slot, VBody &b) {           // velocity phase: SoA records
     b.proc = !(tag & 0x80000000u); b.id = tag & 0x7FFFFFFFu;
     if (b.proc) {
@@ -1701,10 +1733,11 @@ __global__ void __launch_bounds__(TILE_CAP, 2) k_island_tiles(Dev d, int vel_ite
         const uint32_t c0 = d.tile_c0[tile], c1 = min(d.tile_c1[tile], c0 + TILE_CAP), h0 = d.tile_h0[tile], h1 = min(d.tile_h1[tile], h0 + TILE_CAP);
         if (t < 2) s_ncol[t] = 0;
         uint32_t mybody = 0;
-        if (t < nb) {
+        if (t < nb) {       // body state for the row preparation, by slot; the velocities sit where dv, dw go until it ends
             mybody = d.tile_body[(size_t)tile * TILE_CAP + t];
-            s_body[t] = make_float4(0, 0, 0, 0); s_body[TILE_CAP + t] = make_float4(0, 0, 0, 0);
+            s_body[t] = d.linvel[mybody]; s_body[TILE_CAP + t] = d.angvel[mybody];
             s_body[2 * TILE_CAP + t] = d.invIW[3 * mybody]; s_body[3 * TILE_CAP + t] = d.invIW[3 * mybody + 1]; s_body[4 * TILE_CAP + t] = d.invIW[3 * mybody + 2];
+            s_body[5 * TILE_CAP + t] = d.pos[mybody]; s_body[6 * TILE_CAP + t] = d.orn[mybody];
             s_err[t] = 0; s_done[t] = 0; s_root[t] = d.parent[mybody] == mybody ? 1u : 0u;
         }
         __syncthreads();
@@ -1714,24 +1747,36 @@ __global__ void __launch_bounds__(TILE_CAP, 2) k_island_tiles(Dev d, int vel_ite
         uint32_t hcol = 0xFFu, ccol = 0xFFu;
         float4 a0, a1, a2, a3, aim, b0, b1, b2, b3, bim;      // rows of contact points 1 and 2
         a0 = a1 = a2 = a3 = aim = b0 = b1 = b2 = b3 = bim = make_float4(0, 0, 0, 0);
+        // ---- row preparation (k_prepare_hinges / k_prepare_contacts of the tiled range): rows go straight to where the
+        // solve keeps them; hh / ch are the row headers those kernels write (tags, hinge id | point count, body slots)
         if (hasH) {
-            hh = d.hhdr[hi]; hcol = d.hkey_s[hi] & 63u;
-            const float4 *R = d.HR + 7 * (size_t)hi;
-            #pragma unroll
-            for (int k = 0; k < 7; ++k) s_hr[k * TILE_CAP + t] = R[k];
+            const uint32_t h = d.hidx_s[hi];
+            const uint2 pr = d.hpair[h];
+            SBody A, B; v3 posA, posB; q4 ornA, ornB; uint32_t sa, sb;
+            tile_solver_body(d, s_body, pr.x, A, posA, ornA, sa); tile_solver_body(d, s_body, pr.y, B, posB, ornB, sb);
+            hinge_rows(d, h, A, B, posA, ornA, posB, ornB, s_hr + t, TILE_CAP);
+            hh = make_uint4(pr.x | (A.proc ? 0u : 0x80000000u), pr.y | (B.proc ? 0u : 0x80000000u), h, sa | (sb << 16));
+            hcol = d.hkey_s[hi] & 63u;
             atomicMax(&s_ncol[0], hcol + 1u);
         }
         if (hasC) {
-            ch = d.hdr[ci]; ccol = d.ckey_s[ci] & 63u;
-            a0 = d.R0[ci]; a1 = d.R1[ci]; a2 = d.R2[ci]; a3 = d.R3[ci]; aim = d.IMP[ci];
-            if (ch.z > 1) { b0 = d.R0[NM + ci]; b1 = d.R1[NM + ci]; b2 = d.R2[NM + ci]; b3 = d.R3[NM + ci]; bim = d.IMP[NM + ci]; }
-            for (uint32_t s = 2; s < ch.z; ++s) {
-                const size_t ri = s * NM + ci;
+            const uint32_t m = d.cidx_s[ci];
+            const uint2 pr = d.mpair[m];
+            const uint32_t npts = d.mstate[m] & MS_NPTS_MASK;
+            SBody A, B; v3 posA, posB; q4 ornA, ornB; uint32_t sa, sb;
+            tile_solver_body(d, s_body, pr.x, A, posA, ornA, sa); tile_solver_body(d, s_body, pr.y, B, posB, ornB, sb);
+            ch = make_uint4(pr.x | (A.proc ? 0u : 0x80000000u), pr.y | (B.proc ? 0u : 0x80000000u), npts, sa | (sb << 16));
+            contact_point_rows(d, m, A, B, posA, ornA, posB, ornB, a0, a1, a2, a3, aim);
+            if (npts > 1) contact_point_rows(d, NM + m, A, B, posA, ornA, posB, ornB, b0, b1, b2, b3, bim);
+            for (uint32_t s = 2; s < npts; ++s) {
                 float4 *r = s_row + (s - 2) * 5 * TILE_CAP + t;
-                r[0] = d.R0[ri]; r[TILE_CAP] = d.R1[ri]; r[2 * TILE_CAP] = d.R2[ri]; r[3 * TILE_CAP] = d.R3[ri]; r[4 * TILE_CAP] = d.IMP[ri];
+                contact_point_rows(d, s * NM + m, A, B, posA, ornA, posB, ornB, r[0], r[TILE_CAP], r[2 * TILE_CAP], r[3 * TILE_CAP], r[4 * TILE_CAP]);
             }
+            ccol = d.ckey_s[ci] & 63u;
             atomicMax(&s_ncol[1], ccol + 1u);
         }
+        __syncthreads();
+        if (t < nb) { s_body[t] = make_float4(0, 0, 0, 0); s_body[TILE_CAP + t] = make_float4(0, 0, 0, 0); }
         __syncthreads();
         const uint32_t nhc = s_ncol[0], ncc = s_ncol[1];
         // ---- velocity iterations (as in k_solve_tiles)
@@ -1800,12 +1845,12 @@ __global__ void __launch_bounds__(TILE_CAP, 2) k_island_tiles(Dev d, int vel_ite
         a40 = b40 = n40 = l40 = a41 = b41 = n41 = l41 = make_float4(0, 0, 0, 0);
         float4 spos = make_float4(0, 0, 0, 0), sorn = make_float4(0, 0, 0, 1);      // this thread's non-procedural partner (contact, else joint)
         if (hasH) {
-            hisl = d.bslot[d.hisl[hi]];
+            hisl = d.bslot[island_of(d, hh.x & 0x7FFFFFFFu, hh.y & 0x7FFFFFFFu)];
             const uint32_t h = hh.z;
             fA0 = mk3(d.hfA0[h]); fB0 = mk3(d.hfB0[h]); pvA = mk3(d.hpivA[h]); pvB = mk3(d.hpivB[h]);
         }
         if (hasC) {
-            cisl = d.bslot[d.pisl[ci]];
+            cisl = d.bslot[island_of(d, ch.x & 0x7FFFFFFFu, ch.y & 0x7FFFFFFFu)];
             a40 = d.pA[m]; b40 = d.pB[m]; n40 = d.pN[m]; l40 = d.pL[m];
             if (ch.z > 1) { a41 = d.pA[NM + m]; b41 = d.pB[NM + m]; n41 = d.pN[NM + m]; l41 = d.pL[NM + m]; }
         }

@@ -1,0 +1,83 @@
+"""Per-kernel device time of one simulation step of a bench.py workload, from torch.profiler (CUPTI).
+
+    python tools/kernel_times.py WORKLOAD [--steps N] [--warmup W] --out DIR
+
+The scene is built and settled as bench.py does it (same generator, capacity and settle steps).  The step time is
+taken first with CUDA events and the profiler off; then N steps run under torch.profiler with CUDA activities and
+every kernel's summed duration is divided by N.  The world steps without its CUDA graph (B2D_GRAPH=0) so that every
+kernel is its own launch in the trace; kernel durations do not depend on that, the gaps between them do.
+
+Writes DIR/kernel_times_<WORKLOAD>.txt (table, largest first) and DIR/kernel_times_<WORKLOAD>.json."""
+import argparse
+import collections
+import json
+import os
+import sys
+
+os.environ["B2D_GRAPH"] = "0"
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+import bench  # noqa: E402
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("workload")
+    ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--warmup", type=int, default=20)
+    ap.add_argument("--out", required=True)
+    args = ap.parse_args()
+
+    import torch
+    import edyn_b200 as E
+    from torch.profiler import profile, ProfilerActivity
+
+    scene = bench.make_scene(args.workload)
+    w = E.scenes.build_world(scene, device=0, max_manifolds=bench.capacity(args.workload, len(scene["bodies"]["kind"])))
+    w.step(bench.SETTLE_STEPS)
+    w.step(args.warmup)
+    w.sync()
+
+    stream = torch.cuda.ExternalStream(w.stream, device=0)
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record(stream)
+    w.step(args.steps)
+    e1.record(stream)
+    w.sync()
+    step_ms = e0.elapsed_time(e1) / args.steps
+
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        w.step(args.steps)
+        w.sync()
+    per = collections.defaultdict(lambda: [0, 0.0])
+    for ev in prof.events():
+        if ev.device_type != torch.autograd.DeviceType.CUDA:
+            continue
+        name = ev.name.split("(")[0].split("<")[0] or ev.name
+        per[name][0] += 1
+        per[name][1] += ev.time_range.elapsed_us()
+    st = w.stats()
+    w.close()
+    if not per:
+        raise SystemExit("kernel_times: the profiler recorded no device activity")
+
+    rows = sorted(((n, c / args.steps, us / args.steps) for n, (c, us) in per.items()), key=lambda r: -r[2])
+    total_us = sum(r[2] for r in rows)
+    gpu = torch.cuda.get_device_name(0)
+    head = (f"{args.workload} on {gpu}: {args.steps} profiled steps after {bench.SETTLE_STEPS} + {args.warmup} untimed; "
+            f"step {step_ms * 1e3:.1f} us (CUDA events, profiler off, no graph); kernels {total_us:.1f} us per step; "
+            f"{st['contact_points']} contact points, {st['hinges']} hinges, {st['manifolds']} manifolds")
+    lines = [head, f"{'us/step':>10} {'%kern':>6} {'launches':>8}  kernel"]
+    lines += [f"{us:10.1f} {100 * us / total_us:6.1f} {c:8.1f}  {n}" for n, c, us in rows]
+    os.makedirs(args.out, exist_ok=True)
+    with open(os.path.join(args.out, f"kernel_times_{args.workload}.txt"), "w") as f:
+        f.write("\n".join(lines) + "\n")
+    with open(os.path.join(args.out, f"kernel_times_{args.workload}.json"), "w") as f:
+        json.dump({"workload": args.workload, "gpu": gpu, "steps": args.steps, "step_us": step_ms * 1e3, "kernel_us": total_us,
+                   "kernels": [{"name": n, "launches_per_step": c, "us_per_step": us} for n, c, us in rows]}, f, indent=1)
+    print("\n".join(lines))
+
+
+if __name__ == "__main__":
+    main()
