@@ -47,7 +47,8 @@ class Stats(C.Structure):
     _fields_ = [(n, C.c_uint32) for n in ("bodies", "manifolds", "contact_points", "hinges", "contact_colors",
                                          "hinge_colors", "islands", "manifold_high_water")] + \
                [("kernel_launches", C.c_uint64), ("steps", C.c_uint64), ("last_step_ms", C.c_float),
-                ("solve_ms", C.c_float), ("integrate_ms", C.c_float), ("error_flags", C.c_uint32)]
+                ("solve_ms", C.c_float), ("integrate_ms", C.c_float), ("error_flags", C.c_uint32),
+                ("steps_rebuilt", C.c_uint64), ("steps_reused", C.c_uint64)]
 
 
 EXPORTS = ["b2d_create", "b2d_destroy", "b2d_last_error", "b2d_add_bodies", "b2d_remove_bodies", "b2d_wake_bodies", "b2d_download_sleeping", "b2d_add_hinges", "b2d_add_exclusions", "b2d_remove_exclusions",

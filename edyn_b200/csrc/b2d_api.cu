@@ -57,7 +57,12 @@ struct b2d_world {
     // [integration .. refresh].  Captured lazily, dropped whenever a host-side parameter of the sequence changes.
     bool use_graph = true, graph_valid = false;
     cudaGraphExec_t gx_pre = nullptr, gx_solve = nullptr, gx_post = nullptr, gx_all = nullptr;
-    uint64_t graph_launches = 0;      // kernels one replay of the step graphs launches
+    uint64_t graph_launches = 0;      // kernels one replay of the step graphs launches (a skipped island rebuild included)
+    // island rebuild reuse (B2D_GRAPH_REUSE=0 turns it off): the captured step holds the rebuild under a conditional node
+    // that runs it only when Counters::graph_changed is set; the body is captured on its own stream
+    bool graph_reuse = true, graph_cond = false;
+    cudaStream_t body_stream = nullptr;
+    uint64_t host_rebuilt = 0;        // steps that ran the rebuild unconditionally (plain launches, graphs without reuse)
     bool timing = true;               // per-kernel event ring (b2d_get_stats); off = the whole step is one graph
     // multi-GPU hand-over
     std::vector<uint32_t> host_bdst;  // destination rank per body of the current plan
@@ -65,9 +70,11 @@ struct b2d_world {
     uint32_t plan_ranks = 0;
 };
 
+// Something the island rebuild reads changed behind the device kernels' back: the next step rebuilds.
+static void mark_graph_changed(b2d_world *w) { cudaMemsetAsync(&w->d.cnt->graph_changed, 0x01, sizeof(uint32_t), w->stream); }
 // The captured step no longer matches the world (counts, table pointers, grid pitch changed): re-capture before the next
 // replay.  The executable graphs are kept so that the re-capture can patch them in place (capture()).
-static void drop_graphs(b2d_world *w) { w->graph_valid = false; w->cells_dirty = true; }
+static void drop_graphs(b2d_world *w) { w->graph_valid = false; w->cells_dirty = true; mark_graph_changed(w); }
 // B2D_TRACE=1: wall-clock marks of the hand-over entry points on stderr (development aid)
 struct Trace {
     const char *what; bool on; std::chrono::steady_clock::time_point t0;
@@ -161,7 +168,7 @@ b2d_world *b2d_create(const b2d_config *cfg) {
     ok = ok && dalloc(w, d.pA, 4 * (size_t)NM) && dalloc(w, d.pB, 4 * (size_t)NM) && dalloc(w, d.pN, 4 * (size_t)NM);
     ok = ok && dalloc(w, d.pL, 4 * (size_t)NM) && dalloc(w, d.pI, 4 * (size_t)NM) && dalloc(w, d.npres, NM) && dalloc(w, d.clist, NM);
     ok = ok && dalloc(w, d.parent, NB) && dalloc(w, d.bmask, NB) && dalloc(w, d.jmask, NB) && dalloc(w, d.prop, NB) && dalloc(w, d.jprop, NB);
-    ok = ok && dalloc(w, d.ckey, NM) && dalloc(w, d.ckey_s, NM) && dalloc(w, d.cidx, NM) && dalloc(w, d.cidx_s, NM);
+    ok = ok && dalloc(w, d.ckey, NM) && dalloc(w, d.ckey_s, NM) && dalloc(w, d.cidx, NM) && dalloc(w, d.cidx_s, NM) && dalloc(w, d.npidx, NM);
     ok = ok && dalloc(w, d.hkey, NH) && dalloc(w, d.hkey_s, NH) && dalloc(w, d.hidx, NH) && dalloc(w, d.hidx_s, NH);
     // island tiles: the census arrays are one allocation (zeroed together every step), so are the per-tile tables
     d.max_tiles = (uint32_t)std::min<uint64_t>(((uint64_t)NB + NM + NH) / TILE_ISLAND_MAX + 64, 1u << KEY_TILE_BITS);   // beyond: dataflow path
@@ -225,6 +232,8 @@ b2d_world *b2d_create(const b2d_config *cfg) {
     if (const char *e = getenv("B2D_BP_WARP_MAX")) w->bp_warp_max = (uint32_t)std::max(0, atoi(e));
     if (const char *e = getenv("B2D_TILES")) if (atoi(e) == 0) d.max_tiles = 0;          // development: everything through the dataflow path
     if (const char *e = getenv("B2D_GRAPH")) w->use_graph = atoi(e) != 0;
+    if (const char *e = getenv("B2D_GRAPH_REUSE")) w->graph_reuse = atoi(e) != 0;     // 0: graphs rebuild the islands every step
+    if (w->use_graph && w->graph_reuse && cudaStreamCreateWithFlags(&w->body_stream, cudaStreamNonBlocking) != cudaSuccess) { cudaGetLastError(); w->body_stream = nullptr; w->graph_reuse = false; }
 
     if (!ok || cudaStreamSynchronize(w->stream) != cudaSuccess) {
         g_create_error = "b2d_create: device allocation failed: " + w->error;
@@ -243,6 +252,7 @@ void b2d_destroy(b2d_world *w) {
     if (w->ev_step0) cudaEventDestroy(w->ev_step0);
     if (w->ev_step1) cudaEventDestroy(w->ev_step1);
     for (int i = 0; i < b2d_world::RING; ++i) for (cudaEvent_t e : {w->ev_solve0[i], w->ev_solve1[i], w->ev_int0[i], w->ev_int1[i]}) if (e) cudaEventDestroy(e);
+    if (w->body_stream) cudaStreamDestroy(w->body_stream);
     if (w->stream) cudaStreamDestroy(w->stream);
     delete w;
 }
@@ -394,6 +404,7 @@ int b2d_wake_bodies(b2d_world *w, const uint32_t *ids, uint32_t n) {
     cudaSetDevice(w->cfg.device);
     Dev &d = w->d;
     cudaStream_t s = w->stream;
+    mark_graph_changed(w);                              // sleeping flags decide which constraints have rows
     if (!ids) { if (d.nbodies) LAUNCH(k_wake_bodies, d.nbodies, 256, d, (const uint32_t *)nullptr, d.nbodies); CK(cudaStreamSynchronize(s)); return B2D_OK; }
     for (uint32_t k = 0; k < n; ++k) if (ids[k] >= d.nbodies) { w->error = "b2d_wake_bodies: body id out of range"; return B2D_ERR_ARGUMENT; }
     if (!n) return B2D_OK;
@@ -492,6 +503,7 @@ static int insert_exclusions(b2d_world *w, const std::vector<uint64_t> &keys) {
     unsigned long long *tmp = (unsigned long long *)w->stage;
     CK(cudaMemcpyAsync(tmp, keys.data(), keys.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, w->stream));
     LAUNCH(k_xhash_insert, keys.size(), 256, d, (const unsigned long long *)tmp, (uint32_t)keys.size());
+    mark_graph_changed(w);
     CK(cudaStreamSynchronize(w->stream));             // `keys` may go out of scope, the staging buffer be reused
     w->xhash_used += (uint32_t)keys.size();
     return B2D_OK;
@@ -609,12 +621,20 @@ static int enqueue_restitution(b2d_world *w) {
     LAUNCH(k_rest_solve, d.nbodies, 64, d);
     return B2D_OK;
 }
-static int enqueue_solver_a(b2d_world *w, int recolor) {
+static int enqueue_gravity(b2d_world *w) {
+    Dev &d = w->d;
+    if (d.nbodies) LAUNCH(k_gravity, d.nbodies, 256, d);
+    return B2D_OK;
+}
+// The island rebuild after the connected components: census, colouring, tile packing, sort keys, sorts and colour
+// ranges.  A pure function of the constraint graph (and, on the dataflow path, of the spatial ranks and point counts);
+// what it leaves -- parent, btile / bslot, the tile tables, cidx_s / hidx_s, the key arrays and the range counters --
+// stays valid for as long as the graph does not change.
+static int enqueue_rebuild(b2d_world *w, int recolor) {
     Dev &d = w->d; cudaStream_t s = w->stream;
-    { int rc = enqueue_restitution(w); if (rc) return rc; }
     CK(cudaMemsetAsync(d.isl_nb, 0, 3 * (size_t)d.NB * sizeof(uint32_t), s));             // island census: bodies, manifolds, joints
     CK(cudaMemsetAsync(d.tile_nb, 0, 5 * (size_t)d.max_tiles * sizeof(uint32_t), s));      // tile body counts and (empty) ranges
-    LAUNCH(k_gravity, std::max<uint32_t>(d.nbodies, 1), 256, d);                             // + resets of the colouring / packing accumulators
+    LAUNCH(k_island_census, std::max<uint32_t>(d.nbodies, 1), 256, d);                      // + resets of the colouring / packing accumulators
     LAUNCH(k_color_list, d.NM, 256, d, recolor);
     CK(coop_launch(w, k_color, w->coop_blocks_color, 256, d));
     size_t t;
@@ -631,10 +651,19 @@ static int enqueue_solver_a(b2d_world *w, int recolor) {
     CK(cub::DeviceRadixSort::SortPairs(w->cub_tmp, t, d.hkey, d.hkey_s, d.hidx, d.hidx_s, (int)d.NH, 0, COLOR_KEY_BITS, s)); w->launches += 3;
     LAUNCH(k_color_offsets, d.NM, 256, d);
     LAUNCH(k_color_fixup, 1, 32, d);
+    return B2D_OK;
+}
+static int enqueue_prepare(b2d_world *w) {
+    Dev &d = w->d;
     const int fused = (d.max_tiles && w->cfg.position_iterations > 0) ? 1 : 0;        // k_island_tiles prepares the tiled rows
     LAUNCH(k_prepare_contacts, d.NM, 256, d, fused);
     if (d.nhinges) LAUNCH(k_prepare_hinges, d.nhinges, 256, d, fused);
     return B2D_OK;
+}
+static int enqueue_solver_a(b2d_world *w, int recolor) {
+    int rc;
+    if ((rc = enqueue_restitution(w)) || (rc = enqueue_gravity(w)) || (rc = enqueue_rebuild(w, recolor))) return rc;
+    return enqueue_prepare(w);
 }
 static int enqueue_solver_b(b2d_world *w) {
     Dev &d = w->d;
@@ -671,6 +700,7 @@ static int enqueue_solver(b2d_world *w) {
     const int recolor = ((w->cfg.flags & B2D_FLAG_RECOLOR_EACH_STEP) || w->contacts_dirty) ? 1 : 0;
     w->contacts_dirty = false;
     int rc = enqueue_solver_a(w, recolor); if (rc) return rc;
+    ++w->host_rebuilt;
     const int slot = (int)(w->timed_steps % b2d_world::RING);
     if (w->timing) cudaEventRecord(w->ev_solve0[slot], w->stream);
     rc = enqueue_solver_b(w); if (rc) return rc;
@@ -746,10 +776,55 @@ int b2d_run_phases(b2d_world *w, uint32_t mask) {
 }
 
 extern "C++" {
+#ifndef B2D_EMU
+// Capture `body` as the body of a conditional IF node of the graph being captured on w->stream, behind k_rebuild_decide,
+// which opens the node iff Counters::graph_changed is set.  The body goes into the node's own graph through a capture on
+// w->body_stream (the enqueue_* functions launch on w->stream, which points there meanwhile).
+template<typename F>
+static int enqueue_if_changed(b2d_world *w, F body) {
+    cudaStreamCaptureStatus status; cudaGraph_t g = nullptr; const cudaGraphNode_t *deps = nullptr; size_t ndeps = 0;
+    CK(cudaStreamGetCaptureInfo(w->stream, &status, nullptr, &g, &deps, &ndeps));
+    cudaGraphConditionalHandle h;
+    CK(cudaGraphConditionalHandleCreate(&h, g, 1u, cudaGraphCondAssignDefault));      // rebuild unless told otherwise
+    k_rebuild_decide<<<1, 32, 0, w->stream>>>(w->d, h);                                  // control, not counted as a launch
+    CK(cudaGetLastError());
+    CK(cudaStreamGetCaptureInfo(w->stream, &status, nullptr, &g, &deps, &ndeps));
+    cudaGraphNodeParams p = {};
+    p.type = cudaGraphNodeTypeConditional;
+    p.conditional.handle = h; p.conditional.type = cudaGraphCondTypeIf; p.conditional.size = 1;
+    cudaGraphNode_t node;
+    CK(cudaGraphAddNode(&node, g, deps, ndeps, &p));
+    CK(cudaStreamBeginCaptureToGraph(w->body_stream, p.conditional.phGraph_out[0], nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
+    cudaStream_t main = w->stream;
+    w->stream = w->body_stream;
+    const int rc = body();
+    w->stream = main;
+    cudaGraph_t bg = nullptr;
+    const cudaError_t e = cudaStreamEndCapture(w->body_stream, &bg);
+    if (rc) return rc;
+    CK(e);
+    CK(cudaStreamUpdateCaptureDependencies(w->stream, &node, 1, cudaStreamSetCaptureDependencies));
+    return B2D_OK;
+}
+#else
+template<typename F>
+static int enqueue_if_changed(b2d_world *w, F) { w->error = "conditional graph nodes: not in the CPU emulation"; return B2D_ERR_UNSUPPORTED; }
+#endif
+// Everything before the velocity solve, as captured.  With `reuse` (only where the step has neither island sleeping nor
+// the restitution solver) the connected components and the island rebuild sit under a conditional node that skips them
+// while the constraint graph is unchanged; gravity, which neither reads nor writes anything they touch, runs first.
+static int enqueue_front(b2d_world *w, bool reuse) {
+    int rc;
+    if ((rc = enqueue_broadphase(w)) || (rc = enqueue_narrowphase(w))) return rc;
+    if (!reuse) { if ((rc = enqueue_islands(w))) return rc; return enqueue_solver_a(w, 0); }
+    if ((rc = enqueue_gravity(w))) return rc;
+    if ((rc = enqueue_if_changed(w, [&]() { const int r = enqueue_cc(w); return r ? r : enqueue_rebuild(w, 0); }))) return rc;
+    return enqueue_prepare(w);
+}
 // Capture [begin, end) of the step sequence into an executable graph.  Returns false (and leaves the stream usable)
 // if the capture is refused; the caller then falls back to plain launches for good.
 template<typename F>
-static bool capture(b2d_world *w, cudaGraphExec_t &out, F body) {
+static bool capture(b2d_world *w, cudaGraphExec_t &out, bool patchable, F body) {
     const uint64_t launches0 = w->launches, updates0 = w->updates;
     if (cudaStreamBeginCapture(w->stream, cudaStreamCaptureModeThreadLocal) != cudaSuccess) { cudaGetLastError(); return false; }
     const int rc = body();
@@ -758,13 +833,14 @@ static bool capture(b2d_world *w, cudaGraphExec_t &out, F body) {
     w->launches = launches0; w->updates = updates0;                // nothing ran yet
     if (rc != B2D_OK || e != cudaSuccess || !g) { cudaGetLastError(); if (g) cudaGraphDestroy(g); return false; }
     // same kernels in the same order with new arguments / grid sizes (bodies came or went): patch the executable graph in
-    // place, which is much cheaper than instantiating a new one
-    if (out) {
+    // place, which is much cheaper than instantiating a new one.  A graph with a conditional node is instantiated anew:
+    // its new handle has to reach both the node and the kernel that sets it.
+    if (out && patchable) {
         cudaGraphExecUpdateResultInfo info;
         if (cudaGraphExecUpdate(out, g, &info) == cudaSuccess) { cudaGraphDestroy(g); return true; }
         cudaGetLastError();
-        cudaGraphExecDestroy(out); out = nullptr;
     }
+    if (out) { cudaGraphExecDestroy(out); out = nullptr; }
     const bool ok = cudaGraphInstantiate(&out, g, 0) == cudaSuccess;
     cudaGraphDestroy(g);
     if (!ok) { cudaGetLastError(); out = nullptr; }
@@ -772,18 +848,21 @@ static bool capture(b2d_world *w, cudaGraphExec_t &out, F body) {
 }
 static bool build_graphs(b2d_world *w) {
     w->graph_valid = false;
+    const bool reuse = w->graph_reuse && w->body_stream && !w->d.sleeping && !w->d.rest_iters;
     uint64_t n_pre = 0, n_solve = 0, n_post = 0;
     auto counted = [&](uint64_t &n, auto fn) { return [&, fn]() { const uint64_t l0 = w->launches; int rc = fn(); n = w->launches - l0; return rc; }; };
-    bool ok = capture(w, w->gx_pre, counted(n_pre, [&]() { int rc; if ((rc = enqueue_broadphase(w))) return rc; if ((rc = enqueue_narrowphase(w))) return rc;
-                                                            if ((rc = enqueue_islands(w))) return rc; return enqueue_solver_a(w, 0); }));
-    ok = ok && capture(w, w->gx_solve, counted(n_solve, [&]() { return enqueue_solver_b(w); }));
-    ok = ok && capture(w, w->gx_post, counted(n_post, [&]() { return enqueue_solver_c(w); }));
-    ok = ok && capture(w, w->gx_all, [&]() { int rc; if ((rc = enqueue_broadphase(w))) return rc; if ((rc = enqueue_narrowphase(w))) return rc;
-                                             if ((rc = enqueue_islands(w))) return rc; if ((rc = enqueue_solver_a(w, 0))) return rc;
-                                             if ((rc = enqueue_solver_b(w))) return rc; if ((rc = enqueue_integrate(w))) return rc; return enqueue_solver_c(w); });
+    bool ok = capture(w, w->gx_pre, !reuse, counted(n_pre, [&]() { return enqueue_front(w, reuse); }));
+    ok = ok && capture(w, w->gx_solve, true, counted(n_solve, [&]() { return enqueue_solver_b(w); }));
+    ok = ok && capture(w, w->gx_post, true, counted(n_post, [&]() { return enqueue_solver_c(w); }));
+    ok = ok && capture(w, w->gx_all, !reuse, [&]() { int rc; if ((rc = enqueue_front(w, reuse))) return rc;
+                                                     if ((rc = enqueue_solver_b(w))) return rc; if ((rc = enqueue_integrate(w))) return rc; return enqueue_solver_c(w); });
+    // the driver refused the conditional node: graphs that rebuild the islands every step
+    if (!ok && reuse) { destroy_graphs(w); w->graph_reuse = false; return build_graphs(w); }
     if (!ok) { destroy_graphs(w); w->use_graph = false; return false; }
     w->graph_launches = n_pre + n_solve + n_post + 1;
+    w->graph_cond = reuse;
     w->graph_valid = true;
+    mark_graph_changed(w);          // a new capture starts with a rebuild
     return true;
 }
 } // extern "C++"
@@ -814,10 +893,12 @@ int b2d_step(b2d_world *w, uint32_t num_steps) {
             CK(cudaGraphLaunch(w->gx_post, w->stream));
             ++w->timed_steps; w->timed = true; ++w->updates;
             w->launches += w->graph_launches;
+            if (!w->graph_cond) ++w->host_rebuilt;
         } else {
             CK(cudaGraphLaunch(w->gx_all, w->stream));
             ++w->updates;
             w->launches += w->graph_launches;
+            if (!w->graph_cond) ++w->host_rebuilt;
         }
         ++w->steps;
     }
@@ -970,6 +1051,7 @@ int b2d_upload_contacts(b2d_world *w, uint32_t n, const uint32_t *pairs, const u
         }
     }
     CK(cudaMemcpyAsync(&d.cnt->hwm, &n, sizeof(uint32_t), cudaMemcpyHostToDevice, s_));
+    mark_graph_changed(w);
     CK(cudaStreamSynchronize(s_));
     w->contacts_dirty = true;
     return B2D_OK;
@@ -1032,6 +1114,7 @@ int b2d_get_stats(b2d_world *w, b2d_stats *out) {
     out->bodies = d.nbodies; out->manifolds = (uint32_t)hm.slots.size(); out->contact_points = c.npoints; out->hinges = d.nhinges;
     out->contact_colors = c.ncolors_all; out->hinge_colors = c.nhcolors_all; out->islands = c.nislands; out->manifold_high_water = c.hwm;
     out->kernel_launches = w->launches; out->steps = w->steps; out->error_flags = c.err;
+    out->steps_rebuilt = w->host_rebuilt + c.steps_rebuilt; out->steps_reused = c.steps_reused;
     if (w->timed && w->timed_steps) {
         // average over the steps since b2d_reset_timers (at most the ring size)
         const uint64_t cnt = std::min<uint64_t>(w->timed_steps, b2d_world::RING);
@@ -1116,6 +1199,7 @@ int b2d_upload_bodies(b2d_world *w, uint32_t n, const uint32_t *ids, const b2d_b
     q.inv_mass = put(p->inv_mass, n); q.inv_inertia = put(p->inv_inertia, 9 * (size_t)n); q.gravity = put(p->gravity, 3 * (size_t)n);
     q.friction = put(p->friction, n); q.restitution = put(p->restitution, n); q.kind = (const uint32_t *)put(p->kind, n);
     LAUNCH(k_patch_bodies, n, 256, d, dev_ids, n, q);
+    if (p->kind) mark_graph_changed(w);              // body kinds decide the islands and which constraints have rows
     CK(cudaStreamSynchronize(s));                    // the host arrays may be reused by the caller
     if (p->kind) {
         for (uint32_t k = 0; k < n; ++k) w->isdyn[ids[k]] = p->kind[k] == B2D_DYNAMIC ? 1 : 0;

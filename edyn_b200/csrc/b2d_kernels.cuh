@@ -152,6 +152,7 @@ __global__ void k_bp_separate(Dev d) {
                 // a destroyed body takes its graph edges with it (island_manager.cpp:47-66)
                 if (((d.flags[p.x] | d.flags[p.y]) & F_REMOVED) || !intersect(inset(body_box(d, p.x), BP_SEPARATION), body_box(d, p.y))) {
                     d.mstate[m] = COLOR_NONE << MS_COLOR_SHIFT;      // clear_contact_manifold + destroy
+                    d.cnt->graph_changed = 1u;
                     flag = 1;
                 } else {
                     hash_insert(d.mhash_key, d.mhash_val, d.mhash_size, pair_key(p.x, p.y), m);
@@ -210,12 +211,21 @@ __global__ void k_cell_extent(Dev d, int *out6) {
         if ((threadIdx.x & 31) == 0 && mn[k] <= mx[k]) { atomicMin(&out6[k], mn[k]); atomicMax(&out6[3 + k], mx[k]); }
     }
 }
-// First sorted index of every occupied cell -> hash table.
+B2D_D uint32_t key_body(const Dev &d, uint2 pr) {      // the body a constraint is filed under: its (smaller) dynamic one
+    const uint32_t fa = d.flags[pr.x];
+    return (is_dynamic(fa) && !(fa & F_LARGE)) ? pr.x : pr.y;
+}
+// spatial part of a dataflow manifold's sort key (k_color_keys): the key body's rank in the cell order, 14 bits
+B2D_D uint32_t df_spatial(const Dev &d, uint32_t rank) { return (uint32_t)(((unsigned long long)rank << KEY_DF_SPATIAL_BITS) / d.nbodies); }
+// First sorted index of every occupied cell -> hash table.  A body that is not in an island tile and whose spatial
+// rank moved would change a dataflow sort key: the island rebuild has to run.
 __global__ void k_bp_cell_starts(Dev d) {
     GRID_STRIDE(i, d.nbodies) {
         unsigned long long k = d.cellkey_s[i];
         if (k != EMPTY_KEY && (i == 0 || d.cellkey_s[i - 1] != k)) hash_insert(d.chash_key, d.chash_val, d.chash_size, k, i);
-        d.brank[d.cellbody_s[i]] = i;
+        const uint32_t b = d.cellbody_s[i];
+        if (df_spatial(d, d.brank[b]) != df_spatial(d, i) && d.btile[b] == TILE_NONE) d.cnt->graph_changed = 1u;
+        d.brank[b] = i;
     }
 }
 
@@ -376,6 +386,7 @@ __global__ void k_bp_finish(Dev d) {
         Counters &c = *d.cnt;
         c.nnew = bp_nnew(d);
         if (c.nnew > c.nfree) c.hwm = min(d.NM, c.hwm + (c.nnew - c.nfree));
+        if (c.nnew) c.graph_changed = 1u;
     }
 }
 
@@ -475,7 +486,7 @@ __global__ void k_np_keys(Dev d) {
     __syncthreads();
     if (threadIdx.x < 16 && s_hist[threadIdx.x]) atomicAdd(&d.cnt->npcount[threadIdx.x], s_hist[threadIdx.x]);
 }
-// Counting sort by pair type: manifold slots of one type become a contiguous range of cidx_s.  Every CTA takes windows
+// Counting sort by pair type: manifold slots of one type become a contiguous range of npidx.  Every CTA takes windows
 // of 256 consecutive slots, keeps their order inside a type (manifold slots are spatially coherent, the detect kernels
 // gather body data through them) and claims the window's share of each range with one atomic per type; which window
 // comes first is first come first served -- it only decides which thread runs which manifold.
@@ -503,7 +514,7 @@ __global__ void __launch_bounds__(256) k_np_scatter(Dev d) {
             s_base[threadIdx.x] = acc ? atomicAdd(&c.npcursor[threadIdx.x], acc) : 0u;
         }
         __syncthreads();
-        if (key != 0xFFu) d.cidx_s[s_off[key & 15u] + s_base[key & 15u] + s_wcount[warp][key & 15u] + rank] = m;
+        if (key != 0xFFu) d.npidx[s_off[key & 15u] + s_base[key & 15u] + s_wcount[warp][key & 15u] + rank] = m;
         __syncthreads();
     }
 }
@@ -512,7 +523,7 @@ template<int FN>
 B2D_D void np_detect_range(const Dev &d) {
     const uint32_t b = d.cnt->npoff[FN], e = d.cnt->npoff[FN + 1];
     for (uint32_t i = b + blockIdx.x * blockDim.x + threadIdx.x; i < e; i += gridDim.x * blockDim.x) {
-        const uint32_t m = d.cidx_s[i];
+        const uint32_t m = d.npidx[i];
         const uint2 pr = d.mpair[m];
         const uint32_t fa = d.flags[pr.x], fb = d.flags[pr.y];
         CResult res; res.num = 0;
@@ -637,6 +648,10 @@ __global__ void __launch_bounds__(128) k_np_merge(Dev d) {
         }
         for (int s = 0; s < num; ++s) store_point(d, m, s, P[s]);
         d.mstate[m] = (st & ~MS_NPTS_MASK) | (uint32_t)num;
+        // the island rebuild reads whether a manifold has points (colouring, island census) and, on the dataflow path,
+        // its point count (sort key); inside an island tile the count only matters to the solver itself
+        const uint32_t was = st & MS_NPTS_MASK;
+        if ((uint32_t)num != was && (was == 0u || num == 0 || d.btile[key_body(d, pr)] == TILE_NONE)) d.cnt->graph_changed = 1u;
     }
 }
 
@@ -751,6 +766,7 @@ __global__ void k_sleep_apply(Dev d) {
         const uint32_t r = d.parent[i], fl = d.isl_flags[r];
         if (fl & 1u) f &= ~F_SLEEPING;
         if (fl & 4u) { f |= F_SLEEPING; d.linvel[i] = make_float4(0, 0, 0, 0); d.angvel[i] = make_float4(0, 0, 0, 0); }     // put_to_sleep, :541-566
+        if (f != d.flags[i]) d.cnt->graph_changed = 1u;          // a body fell asleep or woke up
         d.flags[i] = f;
         d.prev_label[i] = r;
     }
@@ -764,19 +780,36 @@ __global__ void k_wake_bodies(Dev d, const uint32_t *ids, uint32_t n) {
 
 // apply_gravity, sys/apply_gravity.hpp:12-17
 __global__ void k_gravity(Dev d) {
-    // also resets what the colouring and the tile packing accumulate into (they run after this kernel)
+    GRID_STRIDE(i, d.nbodies) {
+        if (!is_dynamic(d.flags[i])) continue;
+        v3 v = mk3(d.linvel[i]); v += mk3(d.grav[i]) * d.dt;
+        d.linvel[i] = f4(v, 0);
+    }
+}
+// First kernel of the island rebuild after the connected components: resets what the colouring and the tile packing
+// accumulate into (they run after this kernel), counts the dynamic bodies per island and clears the rebuild flag.
+__global__ void k_island_census(Dev d) {
     if (blockIdx.x == 0 && threadIdx.x == 0) {
         Counters &c = *d.cnt;
         c.remaining[0] = c.remaining[1] = 0; c.nlist = 0; c.bar = 0; c.tile_wmax = 0; c.ncolors_all = 0; c.nhcolors_all = 0;
+        c.graph_changed = 0u;
     }
     GRID_STRIDE(i, d.nbodies) {
         d.bmask[i] = 0ULL; d.jmask[i] = 0ULL; d.prop[i] = ~0ULL; d.jprop[i] = ~0ULL;
         if (!is_dynamic(d.flags[i])) continue;
-        v3 v = mk3(d.linvel[i]); v += mk3(d.grav[i]) * d.dt;
-        d.linvel[i] = f4(v, 0);
         island_count(d.isl_nb, d.parent[i]);          // census for the island tiles (zeroed by the host, k_tile_weights)
     }
 }
+#ifndef B2D_EMU
+// Head of the conditional graph node around the island rebuild: run it iff something it reads changed.
+__global__ void k_rebuild_decide(Dev d, cudaGraphConditionalHandle h) {
+    if (blockIdx.x != 0 || threadIdx.x != 0) return;
+    Counters &c = *d.cnt;
+    const bool changed = c.graph_changed != 0u;
+    cudaGraphSetConditional(h, changed ? 1u : 0u);
+    if (changed) ++c.steps_rebuilt; else ++c.steps_reused;
+}
+#endif
 
 // Colours persist from step to step for constraints that keep producing rows, so in steady state only the few
 // manifolds that just gained their first point (and new hinges) enter the colouring rounds.  This pass
@@ -909,10 +942,6 @@ __global__ void k_tile_assign(Dev d) {
         d.btile[i] = tile; d.bslot[i] = slot;
     }
 }
-B2D_D uint32_t key_body(const Dev &d, uint2 pr) {      // the body a constraint is filed under: its (smaller) dynamic one
-    const uint32_t fa = d.flags[pr.x];
-    return (is_dynamic(fa) && !(fa & F_LARGE)) ? pr.x : pr.y;
-}
 // Sort keys.  Tiled constraints first, tile-major then colour; then the dataflow path's constraints by colour, point
 // count (a chunk of 32 manifolds runs the same number of row solves in every lane) and the spatial rank of the
 // manifold's dynamic body (lanes of a chunk touch neighbouring bodies, whose predecessors finish at about the same
@@ -931,8 +960,7 @@ __global__ void k_color_keys(Dev d) {
                 cmax = max(cmax, col + 1u);
                 if (tile != TILE_NONE) key = (tile << 6) | col;
                 else {
-                    const uint32_t sp = (uint32_t)(((unsigned long long)d.brank[b] << KEY_DF_SPATIAL_BITS) / d.nbodies);
-                    key = KEY_DF | (col << KEY_DF_COLOR_SHIFT) | (((st & MS_NPTS_MASK) - 1u) << KEY_DF_SPATIAL_BITS) | sp;
+                    key = KEY_DF | (col << KEY_DF_COLOR_SHIFT) | (((st & MS_NPTS_MASK) - 1u) << KEY_DF_SPATIAL_BITS) | df_spatial(d, d.brank[b]);
                 }
             }
         }

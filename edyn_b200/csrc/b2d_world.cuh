@@ -75,6 +75,11 @@ struct Counters {
     uint32_t hchunk[MAX_COLORS + 2];
     uint32_t npoff[16];              // narrowphase: start of each pair-type range in the type-sorted list
     uint32_t npcount[16], npcursor[16];      // its histogram and scatter cursors (zeroed by the host)
+    // Island rebuild reuse.  graph_changed is set by whatever changes an input of the island rebuild (connected
+    // components, colouring, tile packing, sort keys and sorts: a pure function of the constraint graph) and cleared
+    // by the rebuild; a CUDA-graph step skips the rebuild while it is clear (b2d_api.cu enqueue_front).
+    uint32_t graph_changed;
+    unsigned long long steps_rebuilt, steps_reused;          // graph steps that ran / skipped the rebuild (statistics)
     unsigned long long dbg[16];  // development counters (B2D_DF_PROFILE builds only)
 };
 
@@ -179,6 +184,10 @@ struct Dev {
     uint32_t *rcnt, *roff, *rcur;            // per body: neighbours in the entity graph, start of its list, fill cursor
     uint32_t *radj, *radj_m;                 // neighbour id | 0x80000000 if the adjacency holds a contact manifold; its manifold slot
     uint32_t *rstamp, *rnext;                // breadth-first walk: visit stamp and queue link per body
+
+    // ---- narrowphase: manifold slots sorted by pair type (its own buffer: cidx_s, the solver order, outlives a step
+    // whose island rebuild is skipped)
+    uint32_t *npidx;
 };
 
 } // namespace b2d

@@ -112,6 +112,10 @@ typedef struct b2d_stats {
     float solve_ms;                /* mean CUDA-event time of the velocity-solve kernel per step since b2d_reset_timers */
     float integrate_ms;            /* ... of the integrate kernel (means cover at most the last 256 steps) */
     uint32_t error_flags;          /* device-side overflow flags, 0 if none */
+    /* Steps that ran the island rebuild (connected components, colouring, tile packing, solver order) and steps that
+       reused the previous one because the constraint graph had not changed (CUDA graphs only; B2D_GRAPH_REUSE=0 turns
+       reuse off).  kernel_launches counts the rebuild's kernels either way. */
+    uint64_t steps_rebuilt, steps_reused;
 } b2d_stats;
 
 b2d_world  *b2d_create(const b2d_config *cfg);

@@ -1,11 +1,13 @@
 """Per-kernel device time of one simulation step of a bench.py workload, from torch.profiler (CUPTI).
 
-    python tools/kernel_times.py WORKLOAD [--steps N] [--warmup W] --out DIR
+    python tools/kernel_times.py WORKLOAD [--steps N] [--warmup W] [--graph] --out DIR
 
 The scene is built and settled as bench.py does it (same generator, capacity and settle steps).  The step time is
 taken first with CUDA events and the profiler off; then N steps run under torch.profiler with CUDA activities and
-every kernel's summed duration is divided by N.  The world steps without its CUDA graph (B2D_GRAPH=0) so that every
-kernel is its own launch in the trace; kernel durations do not depend on that, the gaps between them do.
+every kernel's summed duration is divided by N.  By default the world steps without its CUDA graph (B2D_GRAPH=0), so
+every kernel is its own launch in the trace and the island rebuild runs on every step; kernel durations do not depend
+on that, the gaps between them do.  --graph replays the step graph as bench.py does: the rebuild's kernels then only
+appear on the steps that ran it (the header gives how many did).
 
 Writes DIR/kernel_times_<WORKLOAD>.txt (table, largest first) and DIR/kernel_times_<WORKLOAD>.json."""
 import argparse
@@ -14,7 +16,6 @@ import json
 import os
 import sys
 
-os.environ["B2D_GRAPH"] = "0"
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
@@ -26,8 +27,10 @@ def main():
     ap.add_argument("workload")
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=20)
+    ap.add_argument("--graph", action="store_true", help="step through the CUDA graph (island rebuild reuse on)")
     ap.add_argument("--out", required=True)
     args = ap.parse_args()
+    os.environ["B2D_GRAPH"] = "1" if args.graph else "0"
 
     import torch
     import edyn_b200 as E
@@ -47,6 +50,7 @@ def main():
     w.sync()
     step_ms = e0.elapsed_time(e1) / args.steps
 
+    st0 = w.stats()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         w.step(args.steps)
         w.sync()
@@ -65,8 +69,11 @@ def main():
     rows = sorted(((n, c / args.steps, us / args.steps) for n, (c, us) in per.items()), key=lambda r: -r[2])
     total_us = sum(r[2] for r in rows)
     gpu = torch.cuda.get_device_name(0)
+    rebuilt = st["steps_rebuilt"] - st0["steps_rebuilt"]
+    mode = "CUDA graph" if args.graph else "no graph"
     head = (f"{args.workload} on {gpu}: {args.steps} profiled steps after {bench.SETTLE_STEPS} + {args.warmup} untimed; "
-            f"step {step_ms * 1e3:.1f} us (CUDA events, profiler off, no graph); kernels {total_us:.1f} us per step; "
+            f"step {step_ms * 1e3:.1f} us (CUDA events, profiler off, {mode}); island rebuild on {rebuilt} of the {args.steps} "
+            f"profiled steps; kernels {total_us:.1f} us per step; "
             f"{st['contact_points']} contact points, {st['hinges']} hinges, {st['manifolds']} manifolds")
     lines = [head, f"{'us/step':>10} {'%kern':>6} {'launches':>8}  kernel"]
     lines += [f"{us:10.1f} {100 * us / total_us:6.1f} {c:8.1f}  {n}" for n, c, us in rows]
@@ -74,7 +81,7 @@ def main():
     with open(os.path.join(args.out, f"kernel_times_{args.workload}.txt"), "w") as f:
         f.write("\n".join(lines) + "\n")
     with open(os.path.join(args.out, f"kernel_times_{args.workload}.json"), "w") as f:
-        json.dump({"workload": args.workload, "gpu": gpu, "steps": args.steps, "step_us": step_ms * 1e3, "kernel_us": total_us,
+        json.dump({"workload": args.workload, "gpu": gpu, "graph": args.graph, "steps": args.steps, "steps_rebuilt": rebuilt, "step_us": step_ms * 1e3, "kernel_us": total_us,
                    "kernels": [{"name": n, "launches_per_step": c, "us_per_step": us} for n, c, us in rows]}, f, indent=1)
     print("\n".join(lines))
 
