@@ -6,6 +6,7 @@ Host adapter (this package) -> C ABI (include/b2d.h, edyn_b200/libb2d.so) -> han
 from ._lib import B2DError, build  # noqa: F401
 from .rigidbody import (DYNAMIC, KINEMATIC, STATIC, Material, RigidBodyDef, Shape, bodies_soa, box_shape,  # noqa: F401
                         capsule_shape, plane_shape, sphere_shape)
-from .world import (World, attach, clear_collision_exclusion, detach, exclude_collision, make_hinge,  # noqa: F401
-                    make_rigidbody, remove_collision_exclusion, step_simulation, update)
+from .world import (RAY_CAPSULE_SIDE, RAY_FEATURE_NONE, RAY_MISS, RaycastResult, World, attach,  # noqa: F401
+                    clear_collision_exclusion, detach, exclude_collision, make_hinge, make_rigidbody, raycast,
+                    remove_collision_exclusion, step_simulation, update)
 from . import scenes  # noqa: F401

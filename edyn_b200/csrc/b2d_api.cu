@@ -68,6 +68,12 @@ struct b2d_world {
     std::vector<uint32_t> host_bdst;  // destination rank per body of the current plan
     uint32_t *dev_counts = nullptr;   // nranks x 4 counters of the plan
     uint32_t plan_ranks = 0;
+    // raycast index (k_ray_*): allocated by the first raycast, rebuilt when state_epoch moved past ray_epoch.  Every entry
+    // point that can change a body's AABB, shape or the grid parameters bumps state_epoch.
+    uint64_t state_epoch = 1, ray_epoch = 0;
+    RayIndex rx{};
+    bool ray_alloc = false;
+    void *ray_buf = nullptr; size_t ray_buf_bytes = 0;    // host-array path: rays, ignore list and results on the device
 };
 
 // Something the island rebuild reads changed behind the device kernels' back: the next step rebuilds.
@@ -249,6 +255,7 @@ void b2d_destroy(b2d_world *w) {
     if (w->stream) cudaStreamSynchronize(w->stream);
     destroy_graphs(w);
     for (void *p : w->allocs) cudaFree(p);
+    if (w->ray_buf) cudaFree(w->ray_buf);
     if (w->ev_step0) cudaEventDestroy(w->ev_step0);
     if (w->ev_step1) cudaEventDestroy(w->ev_step1);
     for (int i = 0; i < b2d_world::RING; ++i) for (cudaEvent_t e : {w->ev_solve0[i], w->ev_solve1[i], w->ev_int0[i], w->ev_int1[i]}) if (e) cudaEventDestroy(e);
@@ -326,6 +333,7 @@ static int reclassify(b2d_world *w) {
 int b2d_add_bodies(b2d_world *w, const b2d_bodies *b, uint32_t *first_id) {
     if (!w || !b) return B2D_ERR_ARGUMENT;
     cudaSetDevice(w->cfg.device);
+    ++w->state_epoch;
     Dev &d = w->d;
     const uint32_t n = b->count, first = d.nbodies;
     if (first + (uint64_t)n > d.NB) { w->error = "b2d_add_bodies: max_bodies exceeded"; return B2D_ERR_CAPACITY; }
@@ -381,6 +389,7 @@ int b2d_add_bodies(b2d_world *w, const b2d_bodies *b, uint32_t *first_id) {
 int b2d_remove_bodies(b2d_world *w, const uint32_t *ids, uint32_t n) {
     if (!w || (n && !ids)) return B2D_ERR_ARGUMENT;
     cudaSetDevice(w->cfg.device);
+    ++w->state_epoch;
     Dev &d = w->d;
     for (uint32_t k = 0; k < n; ++k) if (ids[k] >= d.nbodies) { w->error = "b2d_remove_bodies: body id out of range"; return B2D_ERR_ARGUMENT; }
     if (!n) return B2D_OK;
@@ -545,7 +554,7 @@ static int enqueue_broadphase(b2d_world *w) {
     CK(cub::DeviceScan::ExclusiveSum(w->cub_tmp, t, d.free_flag, d.free_rank, (int)d.NM, s)); ++w->launches;
     LAUNCH(k_bp_free_list, d.NM, 256, d);
     if (d.nbodies) {
-        LAUNCH(k_bp_cells, d.nbodies, 256, d);
+        LAUNCH(k_bp_cells, d.nbodies, 256, d, d.cellkey, d.cellbody);
         t = w->cub_tmp_bytes;
         CK(cub::DeviceRadixSort::SortPairs(w->cub_tmp, t, d.cellkey, d.cellkey_s, d.cellbody, d.cellbody_s, (int)d.nbodies, 0, w->cell_key_bits, s)); w->launches += 4;
         LAUNCH(k_bp_cell_starts, d.nbodies, 256, d);
@@ -766,6 +775,7 @@ static int prepare_step(b2d_world *w) {
 int b2d_run_phases(b2d_world *w, uint32_t mask) {
     if (!w) return B2D_ERR_ARGUMENT;
     cudaSetDevice(w->cfg.device);
+    ++w->state_epoch;
     int rc = prepare_step(w); if (rc) return rc;
     if (mask & B2D_PHASE_BROAD) if ((rc = enqueue_broadphase(w))) return rc;
     if (mask & B2D_PHASE_NARROW) if ((rc = enqueue_narrowphase(w))) return rc;
@@ -870,6 +880,7 @@ static bool build_graphs(b2d_world *w) {
 int b2d_step(b2d_world *w, uint32_t num_steps) {
     if (!w) return B2D_ERR_ARGUMENT;
     cudaSetDevice(w->cfg.device);
+    ++w->state_epoch;
     int rc = prepare_step(w); if (rc) return rc;
     cudaEventRecord(w->ev_step0, w->stream);
     for (uint32_t i = 0; i < num_steps; ++i) {
@@ -911,6 +922,7 @@ int b2d_step(b2d_world *w, uint32_t num_steps) {
 int b2d_upload_state(b2d_world *w, const float *pos, const float *orn, const float *lv, const float *av) {
     if (!w || !pos || !orn || !lv || !av) return B2D_ERR_ARGUMENT;
     cudaSetDevice(w->cfg.device);
+    ++w->state_epoch;
     Dev &d = w->d; const size_t n = d.nbodies; cudaStream_t s = w->stream;
     float *sp = w->stage, *so = sp + 3 * n, *sl = so + 4 * n, *sa = sl + 3 * n;
     CK(cudaMemcpyAsync(sp, pos, 3 * n * sizeof(float), cudaMemcpyHostToDevice, s));
@@ -1019,6 +1031,7 @@ int b2d_download_contacts(b2d_world *w, uint32_t capacity, uint32_t *pairs, uint
 int b2d_upload_contacts(b2d_world *w, uint32_t n, const uint32_t *pairs, const uint32_t *num, const float *pt18, const uint32_t *ptu2) {
     if (!w) return B2D_ERR_ARGUMENT;
     cudaSetDevice(w->cfg.device);
+    ++w->state_epoch;
     Dev &d = w->d;
     if (n > d.NM) { w->error = "b2d_upload_contacts: max_manifolds exceeded"; return B2D_ERR_CAPACITY; }
     std::vector<uint2> pr(n); std::vector<uint32_t> st(n);
@@ -1170,6 +1183,103 @@ int b2d_device_bounds(b2d_world *w, float *device_out8) {
     return B2D_OK;
 }
 
+// ------------------------------------------------------------------ raycast
+
+// Enqueue the rebuild of the raycast index if the state changed since the last one; the buffers are allocated by the
+// first raycast, so worlds that never query pay nothing.  No host synchronisation (after the first allocation).
+static int ray_index(b2d_world *w) {
+    Dev &d = w->d; RayIndex &x = w->rx; cudaStream_t s = w->stream;
+    if (!w->ray_alloc) {
+        const uint32_t NB = d.NB;
+        x.hsize = pow2_at_least(2ull * NB);
+        const bool ok = dalloc(w, x.key, NB) && dalloc(w, x.key_s, NB) && dalloc(w, x.body, NB) && dalloc(w, x.body_s, NB) &&
+                        dalloc(w, x.hkey, x.hsize, 0xFF) && dalloc(w, x.hval, x.hsize) && dalloc(w, x.extra, (size_t)NB + 1) &&
+                        dalloc(w, x.bounds, 6);
+        if (!ok) return B2D_ERR_CUDA;
+        w->ray_alloc = true;
+    }
+    if (w->ray_epoch == w->state_epoch) return B2D_OK;
+    LAUNCH(k_ray_reset, 1, 32, x);
+    if (d.nbodies) {
+        LAUNCH(k_bp_cells, d.nbodies, 256, d, x.key, x.body);
+        LAUNCH(k_ray_classify, d.nbodies, 256, d, x);
+        size_t t = w->cub_tmp_bytes;
+        CK(cub::DeviceRadixSort::SortPairs(w->cub_tmp, t, x.key, x.key_s, x.body, x.body_s, (int)d.nbodies, 0, w->cell_key_bits, s)); w->launches += 4;
+        CK(cudaMemsetAsync(x.hkey, 0xFF, (size_t)x.hsize * sizeof(unsigned long long), s));
+        LAUNCH(k_ray_cell_starts, d.nbodies, 256, d, x);
+    }
+    CK(cudaGetLastError());
+    w->ray_epoch = w->state_epoch;
+    return B2D_OK;
+}
+// Device scratch of at least `bytes` for the rays of the host-array path and the shared ignore list.
+static void *ray_scratch(b2d_world *w, size_t bytes) {
+    if (bytes <= w->ray_buf_bytes) return w->ray_buf;
+    if (w->ray_buf) { cudaStreamSynchronize(w->stream); cudaFree(w->ray_buf); w->ray_buf = nullptr; w->ray_buf_bytes = 0; }
+    const size_t want = std::max<size_t>(bytes, 1 << 16);
+    if (cudaMalloc(&w->ray_buf, want) != cudaSuccess) { cudaGetLastError(); w->ray_buf = nullptr; w->error = "raycast: cudaMalloc failed"; return nullptr; }
+    w->ray_buf_bytes = want;
+    return w->ray_buf;
+}
+static bool ray_args(b2d_world *w, uint32_t n, const float *p0, const float *p1, const uint32_t *ignore_list, uint32_t nignore) {
+    if (!w) return false;
+    if ((n && (!p0 || !p1)) || (nignore && !ignore_list)) { w->error = "b2d_raycast: missing segment or ignore array"; return false; }
+    return true;
+}
+static std::vector<uint32_t> ray_ignore(const uint32_t *list, uint32_t n) {     // sorted for the kernel's binary search
+    std::vector<uint32_t> v(list, list + n);
+    std::sort(v.begin(), v.end());
+    v.erase(std::unique(v.begin(), v.end()), v.end());
+    return v;
+}
+
+int b2d_raycast(b2d_world *w, uint32_t n, const float *p0, const float *p1, const uint32_t *ignore_body,
+                const uint32_t *ignore_list, uint32_t nignore, uint32_t *body, float *fraction, float *normal, uint32_t *feature) {
+    if (!ray_args(w, n, p0, p1, ignore_list, nignore)) return B2D_ERR_ARGUMENT;
+    cudaSetDevice(w->cfg.device);
+    int rc = ray_index(w); if (rc) return rc;
+    if (!n) return B2D_OK;
+    const std::vector<uint32_t> ign = ray_ignore(ignore_list, nignore);
+    const size_t m = ign.size();
+    uint32_t *buf = (uint32_t *)ray_scratch(w, (13 * (size_t)n + m) * sizeof(uint32_t));
+    if (!buf) return B2D_ERR_CUDA;
+    float *dp0 = (float *)buf, *dp1 = dp0 + 3 * (size_t)n;
+    uint32_t *dib = (uint32_t *)(dp1 + 3 * (size_t)n), *dil = dib + n, *dbody = dil + m;
+    float *dfr = (float *)(dbody + n), *dnrm = dfr + n;
+    uint32_t *dfeat = (uint32_t *)(dnrm + 3 * (size_t)n);
+    cudaStream_t s = w->stream;
+    CK(cudaMemcpyAsync(dp0, p0, 3 * (size_t)n * sizeof(float), cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(dp1, p1, 3 * (size_t)n * sizeof(float), cudaMemcpyHostToDevice, s));
+    if (ignore_body) CK(cudaMemcpyAsync(dib, ignore_body, (size_t)n * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+    if (m) CK(cudaMemcpyAsync(dil, ign.data(), m * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+    LAUNCH(k_ray_cast, n, 128, w->d, w->rx, n, dp0, dp1, ignore_body ? dib : nullptr, m ? dil : nullptr, (uint32_t)m, dbody, dfr, dnrm, dfeat);
+    CK(cudaGetLastError());
+    if (body) CK(cudaMemcpyAsync(body, dbody, (size_t)n * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    if (fraction) CK(cudaMemcpyAsync(fraction, dfr, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, s));
+    if (normal) CK(cudaMemcpyAsync(normal, dnrm, 3 * (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, s));
+    if (feature) CK(cudaMemcpyAsync(feature, dfeat, (size_t)n * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    return B2D_OK;
+}
+
+int b2d_raycast_device(b2d_world *w, uint32_t n, const float *p0, const float *p1, const uint32_t *ignore_body,
+                       const uint32_t *ignore_list, uint32_t nignore, uint32_t *body, float *fraction, float *normal, uint32_t *feature) {
+    if (!ray_args(w, n, p0, p1, ignore_list, nignore)) return B2D_ERR_ARGUMENT;
+    cudaSetDevice(w->cfg.device);
+    int rc = ray_index(w); if (rc) return rc;
+    if (!n) return B2D_OK;
+    const std::vector<uint32_t> ign = ray_ignore(ignore_list, nignore);
+    uint32_t *dil = nullptr;
+    if (!ign.empty()) {
+        dil = (uint32_t *)ray_scratch(w, ign.size() * sizeof(uint32_t));
+        if (!dil) return B2D_ERR_CUDA;
+        CK(cudaMemcpyAsync(dil, ign.data(), ign.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, w->stream));
+    }
+    LAUNCH(k_ray_cast, n, 128, w->d, w->rx, n, p0, p1, ignore_body, dil, (uint32_t)ign.size(), body, fraction, normal, feature);
+    CK(cudaGetLastError());
+    return B2D_OK;
+}
+
 
 int b2d_set_timing(b2d_world *w, int enabled) { if (!w) return B2D_ERR_ARGUMENT; w->timing = enabled != 0; return B2D_OK; }
 
@@ -1178,6 +1288,7 @@ int b2d_set_timing(b2d_world *w, int enabled) { if (!w) return B2D_ERR_ARGUMENT;
 int b2d_upload_bodies(b2d_world *w, uint32_t n, const uint32_t *ids, const b2d_body_patch *p) {
     if (!w || !p || (n && !ids)) return B2D_ERR_ARGUMENT;
     cudaSetDevice(w->cfg.device);
+    ++w->state_epoch;
     Dev &d = w->d;
     if (!n) return B2D_OK;
     for (uint32_t k = 0; k < n; ++k) {
@@ -1284,6 +1395,7 @@ uint64_t b2d_handover_bytes(const uint32_t *c) {
 int b2d_handover_pack(b2d_world *w, uint32_t dst, void *device_blob, uint64_t capacity) {
     if (!w || !device_blob || dst >= w->plan_ranks) return B2D_ERR_ARGUMENT;
     cudaSetDevice(w->cfg.device);
+    ++w->state_epoch;
     Dev &d = w->d; cudaStream_t s = w->stream;
     const uint32_t *c = &w->plan_counts[4 * dst];
     Trace tr("pack");
@@ -1347,6 +1459,7 @@ int b2d_handover_pack(b2d_world *w, uint32_t dst, void *device_blob, uint64_t ca
 int b2d_handover_unpack(b2d_world *w, const void *device_blob, uint64_t bytes, uint32_t *counts_out) {
     if (!w || !device_blob || bytes < sizeof(BlobHeader)) return B2D_ERR_ARGUMENT;
     cudaSetDevice(w->cfg.device);
+    ++w->state_epoch;
     Dev &d = w->d; cudaStream_t s = w->stream;
     BlobHeader h;
     Trace tr("unpack");

@@ -810,4 +810,134 @@ B2D_D void collide(int kindA, float4 A, int kindB, float4 B, const CCtx &c, CRes
     }
 }
 
+// ---------------------------------------------------------------- src/edyn/collision/raycast.cpp
+// shape_raycast for the four shapes.  fraction / normal / feature are the reference's bits (no clamping to [0, 1]: the
+// world query filters), except the capsule hemisphere normal, which is taken at the hit point from the hemisphere centre.
+
+constexpr uint32_t RAY_FEATURE_NONE = 0xFFFFFFFFu;      // B2D_RAY_FEATURE_NONE
+constexpr uint32_t RAY_CAPSULE_SIDE = 2u;               // B2D_RAY_CAPSULE_SIDE
+struct RayHit { bool hit; float fraction; v3 normal; uint32_t feature; };
+
+B2D_D bool intersect_ray_sphere(v3 p0, v3 p1, v3 pos, float radius, float &t) {   // geom.cpp:1276-1305
+    v3 d = p1 - p0, m = p0 - pos;
+    float a = dot(d, d), b = dot(m, d), c = dot(m, m) - radius * radius;
+    if (c > 0 && b > 0) return false;
+    float discr = b * b - a * c;
+    if (discr < 0) return false;
+    t = (-b - sqrtf(discr)) / a;
+    t = 0.0f < t ? t : 0.0f;                                // std::max(scalar(0), t): NaN gives 0
+    return true;
+}
+B2D_D bool closest_point_line_line(v3 p1, v3 q1, v3 p2, v3 q2, float &s, float &t) {   // geom.cpp:46-70
+    v3 d1 = q1 - p1, d2 = q2 - p2, r = p1 - p2;
+    float a = dot(d1, d1), b = dot(d1, d2), c = dot(d1, r), e = dot(d2, d2), f = dot(d2, r);
+    float d = a * e - b * b;
+    if (!(d > EPS)) return false;
+    float d_inv = 1.0f / d;
+    s = (b * f - c * e) * d_inv;
+    t = (a * f - b * c) * d_inv;
+    return true;
+}
+enum { RCYL_INTERSECTS = 0, RCYL_FAR = 1, RCYL_PARALLEL = 2 };
+// geom.cpp:1225-1274.  Returns the kind; normal / dist_sqr are set when it intersects.
+B2D_D int intersect_ray_cylinder(v3 p0, v3 p1, v3 pos, q4 orn, float radius, float half_length, int axis,
+                                 float &fraction_in, float &dist_sqr, v3 &normal) {
+    v3 dir = rotate(orn, axis_vec(axis));
+    v3 v0 = pos + dir * half_length, v1 = pos - dir * half_length;
+    float s, t;
+    if (!closest_point_line_line(v0, v1, p0, p1, s, t)) return RCYL_PARALLEL;
+    float radius_sqr = square(radius);
+    normal = lerp(p0, p1, t) - lerp(v0, v1, s);
+    dist_sqr = length_sqr(normal);
+    if (dist_sqr > radius_sqr) return RCYL_FAR;
+    v3 d = p1 - p0, e = v1 - v0;
+    float dd = dot(d, d), ee = dot(e, e), de = dot(d, e);
+    float delta_sqr = (radius_sqr - dist_sqr) * ee / (dd * ee - de * de);
+    fraction_in = t - sqrtf(delta_sqr);
+    return RCYL_INTERSECTS;
+}
+B2D_D v3 normalize(v3 v) { return v / length(v); }                              // vector3.hpp:231-235
+
+B2D_D RayHit ray_miss() { RayHit r; r.hit = false; r.fraction = SCALAR_MAX; r.normal = mk3(0, 0, 0); r.feature = RAY_FEATURE_NONE; return r; }
+
+B2D_D RayHit raycast_sphere(float4 sp, v3 pos, v3 p0, v3 p1) {                  // raycast.cpp:182-195
+    RayHit r = ray_miss();
+    float t;
+    if (!intersect_ray_sphere(p0, p1, pos, sp.x, t)) return r;
+    r.hit = true; r.fraction = t; r.normal = normalize(lerp(p0, p1, t) - pos);
+    return r;
+}
+B2D_D RayHit raycast_box(float4 sp, v3 pos, q4 orn, v3 p0w, v3 p1w) {           // raycast.cpp:58-109
+    RayHit r = ray_miss();
+    v3 p0 = to_object(p0w, pos, orn), p1 = to_object(p1w, pos, orn), dir = p1 - p0, he = mk3(sp);
+    float t_min = -SCALAR_MAX, t_max = SCALAR_MAX;
+    int face = -1;
+    #pragma unroll
+    for (int i = 0; i < 3; ++i) {
+        const float di = get(dir, i), pi = get(p0, i), hi = get(he, i);
+        if (fabsf(di) < EPS) {
+            if (fabsf(pi) > hi) return r;
+        } else {
+            float d_inv = 1.0f / di;
+            float t1 = (-hi - pi) * d_inv, t2 = (hi - pi) * d_inv;
+            if (t1 > t2) { float x = t1; t1 = t2; t2 = x; }
+            if (t1 > t_min) face = i * 2 + (pi > 0 ? 0 : 1);
+            t_min = t_min < t1 ? t1 : t_min;                   // std::max
+            t_max = t2 < t_max ? t2 : t_max;                   // std::min
+            if (t_min > t_max) return r;
+        }
+    }
+    if (face < 0) return r;                                    // the reference reads get_face_normal(SIZE_MAX) here
+    r.hit = true; r.fraction = t_min; r.normal = rotate(orn, face_normal(face)); r.feature = (uint32_t)face;
+    return r;
+}
+B2D_D RayHit raycast_capsule(float4 sp, v3 pos, q4 orn, v3 p0, v3 p1) {         // raycast.cpp:197-257
+    RayHit r = ray_miss();
+    float u_in = 0, dist_sqr = 0; v3 n = mk3(0, 0, 0);
+    const int kind = intersect_ray_cylinder(p0, p1, pos, orn, sp.x, sp.y, (int)sp.z, u_in, dist_sqr, n);
+    if (kind == RCYL_FAR) return r;
+    v3 v[2]; capsule_vertices(sp, pos, orn, v);
+    v3 cap_dir = v[1] - v[0];
+    int hemi;
+    if (kind == RCYL_PARALLEL) {
+        hemi = dot(p0 - pos, cap_dir) < 0 ? 0 : 1;
+    } else {
+        v3 x = lerp(p0, p1, u_in);
+        float pr0 = dot(x - v[0], cap_dir), pr1 = dot(x - v[1], cap_dir);
+        if (pr0 > 0 && pr1 < 0) {
+            r.hit = true; r.fraction = u_in; r.normal = n / sqrtf(dist_sqr); r.feature = RAY_CAPSULE_SIDE;
+            return r;
+        }
+        hemi = pr0 < 0 ? 0 : 1;
+    }
+    float f;
+    if (!intersect_ray_sphere(p0, p1, v[hemi], sp.x, f)) return r;
+    // the reference takes lerp(p0, p1, u_in) - pos here (raycast.cpp:217-218): the wrong point from the wrong centre
+    r.hit = true; r.fraction = f; r.normal = normalize(lerp(p0, p1, f) - v[hemi]); r.feature = (uint32_t)hemi;
+    return r;
+}
+B2D_D RayHit raycast_plane(float4 sp, v3 p0, v3 p1) {                          // raycast.cpp:356-378
+    RayHit r = ray_miss();
+    v3 n = mk3(sp);
+    v3 c = n * sp.w;
+    float d = dot(p1 - p0, n), e = dot(c - p0, n);
+    if (fabsf(d) < EPS) {
+        if (!(fabsf(e) < EPS)) return r;
+        r.fraction = 0.0f;
+    } else {
+        r.fraction = e / d;
+    }
+    r.hit = true; r.normal = n;
+    return r;
+}
+B2D_D RayHit shape_raycast(int kind, float4 sp, v3 pos, q4 orn, v3 p0, v3 p1) {
+    switch (kind) {
+    case SH_SPHERE: return raycast_sphere(sp, pos, p0, p1);
+    case SH_BOX: return raycast_box(sp, pos, orn, p0, p1);
+    case SH_CAPSULE: return raycast_capsule(sp, pos, orn, p0, p1);
+    case SH_PLANE: return raycast_plane(sp, p0, p1);
+    default: return ray_miss();
+    }
+}
+
 } // namespace b2d

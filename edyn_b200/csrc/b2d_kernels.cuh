@@ -186,13 +186,14 @@ B2D_D void cell_of(const Dev &d, uint32_t i, int &cx, int &cy, int &cz) {
     cz = (int)floorf((a.z + b.z) * 0.5f * d.inv_cell);
 }
 
-// Cell key per body.  Shapeless and "large" bodies get the all-ones key and sort to the end.
-__global__ void k_bp_cells(Dev d) {
+// Cell key per body.  Shapeless and "large" bodies get the all-ones key and sort to the end.  The broadphase writes
+// d.cellkey / d.cellbody; the raycast index (k_ray_*) its own arrays.
+__global__ void k_bp_cells(Dev d, unsigned long long *cellkey, uint32_t *cellbody) {
     GRID_STRIDE(i, d.nbodies) {
         uint32_t f = d.flags[i];
         unsigned long long key = EMPTY_KEY;
         if (shape_of(f) != SH_NONE && !(f & F_LARGE)) { int cx, cy, cz; cell_of(d, i, cx, cy, cz); key = cell_key_of(d, cx, cy, cz); }
-        d.cellkey[i] = key; d.cellbody[i] = i;
+        cellkey[i] = key; cellbody[i] = i;
     }
 }
 // Cells occupied by the bodies that go into the grid (host: sizes the key fields, b2d_api.cu measure_cells)
@@ -2431,6 +2432,158 @@ __global__ void k_rest_solve(Dev d) {
                 }
             }
         }
+    }
+}
+
+// ====================================================================== raycast (edyn::raycast, src/edyn/collision/raycast.cpp:20-56)
+// Batched segment queries against the current AABBs (DESIGN.md §2b).  The index is the broadphase's uniform grid
+// rebuilt into buffers of its own: bodies are binned by AABB centre with the broadphase's pitch and cell key (so the keys
+// clamp the same way outside the measured extent), and a segment visits every cell within one cell of a cell it passes
+// through.  A grid body's AABB spans at most one pitch per axis, so every point of it lies within one cell of its centre's
+// cell; bodies that do not (large bodies, planes, bodies added since the last classification) are tested brute force.
+// Nothing here writes anything a step reads.
+
+struct RayIndex {
+    unsigned long long *key, *key_s;     // per body: cell key (EMPTY_KEY = not in the grid), sorted
+    uint32_t *body, *body_s;
+    unsigned long long *hkey; uint32_t *hval; uint32_t hsize;   // cell key -> first sorted index
+    uint32_t *extra;                     // [0] count, [1 ..] the bodies outside the grid (k_ray_classify)
+    int *bounds;                         // 6: order-preserving min / max over the grid bodies' AABBs
+};
+constexpr uint32_t RAY_MISS = 0xFFFFFFFFu;   // B2D_RAY_MISS
+
+__global__ void k_ray_reset(RayIndex x) {
+    if (blockIdx.x == 0 && threadIdx.x < 6) x.bounds[threadIdx.x] = threadIdx.x < 3 ? f2ord(INFINITY) : f2ord(-INFINITY);
+    if (blockIdx.x == 0 && threadIdx.x == 6) x.extra[0] = 0;
+}
+// After k_bp_cells: the brute-force list holds the broadphase's large bodies (F_LARGE, planes included) and every body
+// whose AABB is wider than the pitch on some axis (the classification runs before a step; bodies may have been added or
+// patched since).  The grid bodies' AABBs bound the walk.
+__global__ void k_ray_classify(Dev d, RayIndex x) {
+    float mn[3] = {INFINITY, INFINITY, INFINITY}, mx[3] = {-INFINITY, -INFINITY, -INFINITY};
+    GRID_STRIDE(i, d.nbodies) {
+        const uint32_t f = d.flags[i];
+        if (shape_of(f) == SH_NONE) continue;
+        const float4 a = d.bbmin[i], b = d.bbmax[i];
+        if ((f & F_LARGE) || !(b.x - a.x <= d.cell && b.y - a.y <= d.cell && b.z - a.z <= d.cell)) {
+            x.key[i] = EMPTY_KEY;
+            x.extra[1 + atomicAdd(&x.extra[0], 1u)] = i;
+            continue;
+        }
+        mn[0] = fminf(mn[0], a.x); mn[1] = fminf(mn[1], a.y); mn[2] = fminf(mn[2], a.z);
+        mx[0] = fmaxf(mx[0], b.x); mx[1] = fmaxf(mx[1], b.y); mx[2] = fmaxf(mx[2], b.z);
+    }
+    #pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        for (int o = 16; o > 0; o >>= 1) { mn[k] = fminf(mn[k], __shfl_xor_sync(0xffffffffu, mn[k], o)); mx[k] = fmaxf(mx[k], __shfl_xor_sync(0xffffffffu, mx[k], o)); }
+        if ((threadIdx.x & 31) == 0 && mn[k] <= mx[k]) { atomicMin(&x.bounds[k], f2ord(mn[k])); atomicMax(&x.bounds[3 + k], f2ord(mx[k])); }
+    }
+}
+__global__ void k_ray_cell_starts(Dev d, RayIndex x) {
+    GRID_STRIDE(i, d.nbodies) {
+        const unsigned long long k = x.key_s[i];
+        if (k != EMPTY_KEY && (i == 0 || x.key_s[i - 1] != k)) hash_insert(x.hkey, x.hval, x.hsize, k, i);
+    }
+}
+
+struct RayBest { float f; uint32_t id, feature; v3 n; };
+struct RayQuery { v3 p0, p1; uint32_t ignore1; const uint32_t *ignore; uint32_t nignore; };
+
+B2D_D bool ray_ignored(const RayQuery &q, uint32_t j) {
+    if (j == q.ignore1) return true;
+    uint32_t lo = 0, hi = q.nignore;                // sorted shared list
+    while (lo < hi) { const uint32_t m = (lo + hi) >> 1; if (q.ignore[m] < j) lo = m + 1; else hi = m; }
+    return lo < q.nignore && q.ignore[lo] == j;
+}
+// One candidate.  No AABB cull in front of shape_raycast: on long segments the reference's arithmetic (the sphere
+// quadratic above all) can report a hit some way off the shape, and the brute force would report it too.
+B2D_D void ray_test(const Dev &d, const RayQuery &q, uint32_t j, RayBest &b) {
+    const uint32_t f = d.flags[j];
+    const int kind = shape_of(f);
+    if (kind == SH_NONE || ray_ignored(q, j)) return;
+    const RayHit h = shape_raycast(kind, d.shp[j], mk3(d.pos[j]), mkq(d.orn[j]), q.p0, q.p1);
+    if (!h.hit || !(h.fraction >= 0.0f && h.fraction <= 1.0f)) return;
+    if (h.fraction < b.f || (h.fraction == b.f && j < b.id)) { b.f = h.fraction; b.id = j; b.feature = h.feature; b.n = h.normal; }
+}
+B2D_D void ray_probe(const Dev &d, const RayIndex &x, const RayQuery &q, int cx, int cy, int cz, RayBest &b) {
+    const unsigned long long key = cell_key_of(d, cx, cy, cz);
+    uint32_t start;
+    if (!hash_find(x.hkey, x.hval, x.hsize, key, start)) return;
+    for (uint32_t k = start; k < d.nbodies && x.key_s[k] == key; ++k) ray_test(d, q, x.body_s[k], b);
+}
+B2D_D int ray_cell(float v, float inv_cell) { return (int)floorf(fminf(fmaxf(v * inv_cell, -1e9f), 1e9f)); }
+B2D_D bool finite3(v3 v) { return fabsf(v.x) <= FLT_MAX && fabsf(v.y) <= FLT_MAX && fabsf(v.z) <= FLT_MAX; }
+
+// The grid part of one query: clip the segment to the grid bodies' bounds (inflated by half a pitch), then a 3-D DDA
+// (Amanatides & Woo) over the cells it passes.  The first cell probes its 27-cell neighbourhood; a step along axis a
+// adds the 9 cells of the new far layer.  The walk stops once the best fraction lies before the current cell's exit: a
+// body not probed yet has its centre more than one cell from every cell visited, so its surface is at least half a
+// pitch beyond them.
+B2D_D void ray_walk(const Dev &d, const RayIndex &x, const RayQuery &q, RayBest &b) {
+    v3 lo = mk3(ord2f(x.bounds[0]), ord2f(x.bounds[1]), ord2f(x.bounds[2]));
+    v3 hi = mk3(ord2f(x.bounds[3]), ord2f(x.bounds[4]), ord2f(x.bounds[5]));
+    if (!(lo.x <= hi.x && lo.y <= hi.y && lo.z <= hi.z)) return;      // no grid bodies
+    const float pad = 0.5f * d.cell;
+    lo = lo - mk3(pad, pad, pad); hi = hi + mk3(pad, pad, pad);
+    const v3 dir = q.p1 - q.p0;
+    float ta = 0.0f, tb = 1.0f;
+    #pragma unroll
+    for (int a = 0; a < 3; ++a) {
+        const float o = get(q.p0, a), dd = get(dir, a), l = get(lo, a), h = get(hi, a);
+        if (dd == 0.0f) { if (o < l || o > h) return; continue; }
+        float t0 = (l - o) / dd, t1 = (h - o) / dd;
+        if (t0 > t1) { const float s = t0; t0 = t1; t1 = s; }
+        ta = fmaxf(ta, t0); tb = fminf(tb, t1);
+    }
+    if (!(ta <= tb)) return;
+    const v3 s = q.p0 + dir * ta, e = q.p0 + dir * tb;
+    // the parameter where the segment leaves cell c along axis a, from the cell index every time (an incremental
+    // t += cell / |dir| drifts by a good fraction of a cell over thousands of cells)
+    auto exit_t = [&](int a, int ca, int sa) { return ((float)(ca + (sa > 0 ? 1 : 0)) * d.cell - get(q.p0, a)) / get(dir, a); };
+    int c[3], step[3], left[3]; float tnext[3];
+    #pragma unroll
+    for (int a = 0; a < 3; ++a) {
+        c[a] = ray_cell(get(s, a), d.inv_cell);
+        const int ce = ray_cell(get(e, a), d.inv_cell);
+        step[a] = ce > c[a] ? 1 : (ce < c[a] ? -1 : 0);
+        left[a] = ce > c[a] ? ce - c[a] : c[a] - ce;
+        tnext[a] = step[a] ? exit_t(a, c[a], step[a]) : INFINITY;
+    }
+    for (int i = -1; i <= 1; ++i) for (int j = -1; j <= 1; ++j) for (int k = -1; k <= 1; ++k) ray_probe(d, x, q, c[0] + i, c[1] + j, c[2] + k, b);
+    for (;;) {
+        int a = -1; float t = INFINITY;
+        #pragma unroll
+        for (int k = 0; k < 3; ++k) if (left[k] > 0 && (a < 0 || tnext[k] < t)) { a = k; t = tnext[k]; }
+        if (a < 0 || b.f < t) return;
+        c[a] += step[a]; --left[a]; tnext[a] = exit_t(a, c[a], step[a]);
+        const int u = (a + 1) % 3, v = (a + 2) % 3;
+        int p[3]; p[a] = c[a] + step[a];
+        for (int i = -1; i <= 1; ++i) for (int j = -1; j <= 1; ++j) {
+            p[u] = c[u] + i; p[v] = c[v] + j;
+            ray_probe(d, x, q, p[0], p[1], p[2], b);
+        }
+    }
+}
+
+// One thread per segment.  Zero-length and non-finite segments hit nothing.  Any output may be NULL.
+__global__ void k_ray_cast(Dev d, RayIndex x, uint32_t n, const float *p0, const float *p1, const uint32_t *ignore_body,
+                           const uint32_t *ignore, uint32_t nignore, uint32_t *out_body, float *out_fraction, float *out_normal,
+                           uint32_t *out_feature) {
+    GRID_STRIDE(r, n) {
+        RayQuery q;
+        q.p0 = mk3(p0[3 * r], p0[3 * r + 1], p0[3 * r + 2]); q.p1 = mk3(p1[3 * r], p1[3 * r + 1], p1[3 * r + 2]);
+        q.ignore1 = ignore_body ? ignore_body[r] : RAY_MISS; q.ignore = ignore; q.nignore = nignore;
+        RayBest b; b.f = SCALAR_MAX; b.id = RAY_MISS; b.feature = RAY_FEATURE_NONE; b.n = mk3(0, 0, 0);
+        const bool degenerate = q.p0.x == q.p1.x && q.p0.y == q.p1.y && q.p0.z == q.p1.z;
+        if (!degenerate && finite3(q.p0) && finite3(q.p1)) {
+            const uint32_t ne = x.extra[0];
+            for (uint32_t k = 0; k < ne; ++k) ray_test(d, q, x.extra[1 + k], b);
+            ray_walk(d, x, q, b);
+        }
+        if (out_body) out_body[r] = b.id;
+        if (out_fraction) out_fraction[r] = b.f;
+        if (out_normal) { out_normal[3 * r] = b.n.x; out_normal[3 * r + 1] = b.n.y; out_normal[3 * r + 2] = b.n.z; }
+        if (out_feature) out_feature[r] = b.feature;
     }
 }
 

@@ -4,6 +4,7 @@
 //     edyn::make_rigidbody             src/edyn/util/rigidbody.cpp:47-185
 //     edyn::make_hinge (make_constraint<hinge_constraint> + set_axes)   include/edyn/util/constraint_util.hpp:38-54
 //     edyn::exclude_collision          src/edyn/util/exclude_collision.cpp
+//     edyn::raycast                    src/edyn/collision/raycast.cpp:20-56
 //     edyn::update / step_simulation   src/edyn/edyn.cpp:233-273, stepper_sequential.cpp:28-147
 //     edyn::set_fixed_dt / set_solver_velocity_iterations / set_solver_position_iterations
 // EnTT is not available in this image, so the "registry" here is a minimal component store with the same component
@@ -169,6 +170,26 @@ inline void make_hinge(registry &r, entity a, entity b, vector3 pivot_a, vector3
     detail::check(r, b2d_add_hinges(r.world, 1, &a, &b, pa, pb, xa, xb), "b2d_add_hinges");
 }
 inline void exclude_collision(registry &r, entity a, entity b) { detail::check(r, b2d_add_exclusions(r.world, 1, &a, &b), "b2d_add_exclusions"); }
+
+// edyn::raycast_result (include/edyn/collision/raycast.hpp:103-136).  info: box face index, capsule hemisphere index or
+// B2D_RAY_CAPSULE_SIDE, B2D_RAY_FEATURE_NONE for spheres, planes and misses; entity == null on a miss.
+struct raycast_result {
+    scalar fraction{3.402823466e+38f};                  // EDYN_SCALAR_MAX on a miss
+    vector3 normal{};
+    std::uint32_t info{B2D_RAY_FEATURE_NONE};
+    edyn::entity entity{null};
+};
+// edyn::raycast(registry, p0, p1, ignore_entities) (src/edyn/collision/raycast.cpp:20-56); semantics in include/b2d.h.
+inline raycast_result raycast(registry &r, vector3 p0, vector3 p1, const std::vector<entity> &ignore_entities = {}) {
+    if (r.dirty) { detail::check(r, b2d_upload_state(r.world, r.position.data(), r.orientation.data(), r.linvel.data(), r.angvel.data()), "b2d_upload_state"); r.dirty = false; }
+    const float a[3] = {p0.x, p0.y, p0.z}, b[3] = {p1.x, p1.y, p1.z};
+    float n[3];
+    raycast_result res;
+    detail::check(r, b2d_raycast(r.world, 1, a, b, nullptr, ignore_entities.empty() ? nullptr : ignore_entities.data(),
+                                 std::uint32_t(ignore_entities.size()), &res.entity, &res.fraction, n, &res.info), "b2d_raycast");
+    res.normal = {n[0], n[1], n[2]};
+    return res;
+}
 
 // registry.destroy(entity) of a rigid body: its manifolds and joints go with it (island_manager.cpp:47-66); ids are not reused.
 inline void destroy_rigidbody(registry &r, entity e) { detail::check(r, b2d_remove_bodies(r.world, &e, 1), "b2d_remove_bodies"); }

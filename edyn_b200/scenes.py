@@ -215,3 +215,24 @@ def build_world(scene, device=0, max_manifolds=None, flags=0, max_bodies=None, m
     if scene["exclusions"] is not None:
         w.add_exclusions(*scene["exclusions"])
     return w
+
+
+def raycast_segments(lo, hi, n, kind="mixed", seed=0):
+    """Segments over a scene whose bodies lie in the box [lo, hi] (3 floats each): "down" = probes from 1 m above the box
+    to 1 m below it at uniform (x, z), as ground / line-of-sight probes; "across" = horizontal segments at uniform height
+    and heading that cross the whole box; "mixed" = half of each.  Returns p0, p1 as (n, 3) float32."""
+    rng = np.random.default_rng(seed)
+    lo, hi = np.asarray(lo, np.float64), np.asarray(hi, np.float64)
+    nd = n if kind == "down" else (0 if kind == "across" else n // 2)
+    p0, p1 = np.empty((n, 3)), np.empty((n, 3))
+    xz = rng.uniform(lo[[0, 2]], hi[[0, 2]], (nd, 2))
+    p0[:nd] = np.stack([xz[:, 0], np.full(nd, hi[1] + 1.0), xz[:, 1]], 1)
+    p1[:nd] = np.stack([xz[:, 0], np.full(nd, lo[1] - 1.0), xz[:, 1]], 1)
+    na = n - nd
+    c, half = (lo + hi) / 2, np.linalg.norm((hi - lo)[[0, 2]]) / 2 + 1.0
+    ang = rng.uniform(0, 2 * np.pi, na)
+    d = np.stack([np.cos(ang), np.zeros(na), np.sin(ang)], 1)
+    off = rng.uniform(lo[[0, 2]], hi[[0, 2]], (na, 2)) - c[[0, 2]]
+    mid = np.stack([c[0] + off[:, 0] * 0.5, rng.uniform(lo[1], hi[1], na), c[2] + off[:, 1] * 0.5], 1)
+    p0[nd:], p1[nd:] = mid - d * half, mid + d * half
+    return p0.astype(f32), p1.astype(f32)

@@ -25,6 +25,9 @@ PH_BROAD, PH_NARROW, PH_ISLANDS, PH_SOLVE, PH_ALL = 1, 2, 4, 8, 15
 FLAG_RECOLOR_EACH_STEP = 1
 FLAG_RESTITUTION_SOLVER = 4     # the reference's default restitution solver (8 x 3 iterations) instead of restitution through the row rhs
 FLAG_SLEEPING = 2                # island sleeping; off = every body is sleeping_disabled (benchmark configurations)
+RAY_MISS = 0xFFFFFFFF            # B2D_RAY_MISS
+RAY_FEATURE_NONE = 0xFFFFFFFF    # B2D_RAY_FEATURE_NONE
+RAY_CAPSULE_SIDE = 2             # B2D_RAY_CAPSULE_SIDE
 
 
 def _p(a):
@@ -262,6 +265,33 @@ class World:
         self._check(self.l.b2d_download_hinge_impulses(self.h, _p(imp)))
         return imp[:self.num_hinges]
 
+    # -- queries (include/b2d.h, b2d_raycast: semantics)
+    def raycast(self, p0, p1, ignore=None, ignore_body=None) -> dict:
+        """edyn::raycast for n segments at once: p0, p1 are (n, 3).  ignore: body ids no segment may hit; ignore_body: one id
+        per segment (B2D_RAY_MISS for none).  Returns body (n,) uint32 (RAY_MISS on a miss), fraction (n,) float32 (FLT_MAX on a
+        miss), normal (n, 3) float32 and feature (n,) uint32."""
+        a, b = _c(p0, f32), _c(p1, f32)
+        a, b = a.reshape(-1, 3), b.reshape(-1, 3)
+        n = len(a)
+        if b.shape != a.shape:
+            raise ValueError("raycast: p0 and p1 must have the same (n, 3) shape")
+        ign = _c(ignore if ignore is not None else [], u32).reshape(-1)
+        ib = _c(ignore_body, u32, (n,)) if ignore_body is not None else None
+        out = dict(body=np.empty(n, u32), fraction=np.empty(n, f32), normal=np.empty((n, 3), f32), feature=np.empty(n, u32))
+        self._check(self.l.b2d_raycast(self.h, C.c_uint32(n), _p(a), _p(b), _p(ib), _p(ign) if len(ign) else None,
+                                       C.c_uint32(len(ign)), _p(out["body"]), _p(out["fraction"]), _p(out["normal"]), _p(out["feature"])))
+        return out
+
+    def raycast_device(self, n, p0_ptr, p1_ptr, body_ptr=0, fraction_ptr=0, normal_ptr=0, feature_ptr=0, ignore=None,
+                       ignore_body_ptr=0):
+        """Enqueue a raycast of n segments on the world's stream: every argument but `ignore` (host body ids) is an integer
+        DEVICE address (0 = none; p0 / p1 are n x 3 float32, normal n x 3 float32, the rest n words)."""
+        ign = _c(ignore if ignore is not None else [], u32).reshape(-1)
+        v = lambda x: C.c_void_p(x or None)       # noqa: E731
+        self._check(self.l.b2d_raycast_device(self.h, C.c_uint32(n), v(p0_ptr), v(p1_ptr), v(ignore_body_ptr),
+                                              _p(ign) if len(ign) else None, C.c_uint32(len(ign)), v(body_ptr),
+                                              v(fraction_ptr), v(normal_ptr), v(feature_ptr)))
+
     def device_bounds(self, device_ptr):
         """Enqueue the dynamic-AABB bounds reduction into 8 floats (min, max, speed, 0) at `device_ptr` (an int device address)."""
         self._check(self.l.b2d_device_bounds(self.h, C.c_void_p(device_ptr)))
@@ -360,6 +390,25 @@ def clear_collision_exclusion(world: World, e):
     mine = [p for p in world.exclusions if e in p]
     if mine:
         world.remove_exclusions([p[0] for p in mine], [p[1] for p in mine])
+
+
+class RaycastResult:
+    """edyn::raycast_result (include/edyn/collision/raycast.hpp:103-136): entity is the body id (None on a miss), info the
+    feature (box face, capsule hemisphere index or RAY_CAPSULE_SIDE; None for spheres, planes and misses)."""
+
+    def __init__(self, entity, fraction, normal, info):
+        self.entity, self.fraction, self.normal, self.info = entity, fraction, normal, info
+
+    def __repr__(self):
+        return f"RaycastResult(entity={self.entity}, fraction={self.fraction}, normal={self.normal}, info={self.info})"
+
+
+def raycast(world: World, p0, p1, ignore_entities=()) -> RaycastResult:
+    """edyn::raycast(registry, p0, p1, ignore_entities) (src/edyn/collision/raycast.cpp:20-56) for one segment."""
+    r = world.raycast(np.asarray(p0, f32).reshape(1, 3), np.asarray(p1, f32).reshape(1, 3), ignore=list(ignore_entities))
+    body, feat = int(r["body"][0]), int(r["feature"][0])
+    return RaycastResult(None if body == RAY_MISS else body, float(r["fraction"][0]), r["normal"][0].copy(),
+                         None if feat == RAY_FEATURE_NONE else feat)
 
 
 def step_simulation(world: World):

@@ -230,6 +230,35 @@ uint64_t b2d_handover_bytes(const uint32_t *counts4);
 int b2d_handover_pack(b2d_world *w, uint32_t dst, void *device_blob, uint64_t capacity);
 int b2d_handover_unpack(b2d_world *w, const void *device_blob, uint64_t bytes, uint32_t *counts_out);
 
+/* ---- Raycast: edyn::raycast(registry, p0, p1, ignore_entities) (include/edyn/collision/raycast.hpp:157-168,
+ * src/edyn/collision/raycast.cpp:20-56) for a batch of n segments p0[i] -> p1[i] (3 floats each).
+ *   Candidates  every body with a shape that is not removed and not ignored: dynamic, kinematic, static and sleeping.
+ *   Hit         the reference's shape_raycast (raycast.cpp:58-109 box, :182-195 sphere, :197-257 capsule, :356-378 plane)
+ *               gives a fraction f per body; it counts if 0 <= f <= 1 (NaN never does).  The answer is the body with the
+ *               smallest f; equal fractions (==) go to the smaller body id.  So the result is the brute-force minimum over
+ *               all candidates, whatever the spatial index does.  fraction, normal and feature are the reference's bits,
+ *               except the capsule hemisphere normal: normalize(lerp(p0, p1, f) - hemisphere centre).  Consequences: a
+ *               segment that starts inside a sphere reports it at 0; one that starts inside a box or a capsule's side
+ *               reports nothing from that body; a zero-length segment, or one with a non-finite coordinate, hits nothing.
+ *   State       what every step, upload, add or remove enqueued before it on the world's stream left, with the AABBs
+ *               b2d_download_state returns.  A raycast writes nothing a step reads.
+ *   Output      body: local id or B2D_RAY_MISS; fraction: FLT_MAX on a miss; normal: 3 floats, zero on a miss (NaN
+ *               where the reference's is: a segment through a sphere's centre or a capsule's axis);
+ *               feature: box face 0-5 (box_raycast_info), capsule hemisphere 0 / 1 or B2D_RAY_CAPSULE_SIDE
+ *               (capsule_raycast_info), B2D_RAY_FEATURE_NONE for spheres, planes and misses.  Any output may be NULL.
+ *   Ignoring    ignore_list: nignore body ids ignored by every segment (host array, may be NULL when nignore = 0);
+ *               ignore_body: n ids, one per segment (e.g. the agent casting it), or NULL.
+ * b2d_raycast takes and returns HOST arrays and returns when the results are there.  b2d_raycast_device takes DEVICE
+ * pointers for p0 .. feature (ignore_list stays a host array) and only enqueues the work on b2d_stream(w). */
+#define B2D_RAY_MISS 0xFFFFFFFFu
+#define B2D_RAY_FEATURE_NONE 0xFFFFFFFFu
+#define B2D_RAY_CAPSULE_SIDE 2u
+int b2d_raycast(b2d_world *w, uint32_t n, const float *p0, const float *p1, const uint32_t *ignore_body,
+                const uint32_t *ignore_list, uint32_t nignore, uint32_t *body, float *fraction, float *normal, uint32_t *feature);
+int b2d_raycast_device(b2d_world *w, uint32_t n, const float *p0, const float *p1, const uint32_t *ignore_body,
+                       const uint32_t *ignore_list, uint32_t nignore, uint32_t *body, float *fraction, float *normal,
+                       uint32_t *feature);
+
 /* Per-kernel CUDA-event timing of the velocity solve and the integrator (b2d_get_stats).  On (default): a step is
  * replayed as three CUDA graphs with the events in between; off: as one graph. */
 int b2d_set_timing(b2d_world *w, int enabled);
