@@ -28,7 +28,7 @@ struct b2d_world {
     std::string error;
     int num_sms = 0;
     int coop_blocks_color = 0, coop_blocks_df = 0, coop_blocks_pos_df = 0;
-    int tile_blocks = 0, tile_fused_blocks = 0;     // grids of the island-tile kernels (CTAs loop over the tiles)
+    int tile_blocks = 0, tile_fused_blocks = 0, tile_fused_blocks_2p = 0;     // grids of the island-tile kernels (CTAs loop over the tiles)
     int cell_key_bits = 48;                         // sum of d.cell_bits: end bit of the cell sort
     uint32_t bp_warp_max = 100000;                  // neighbourhood search: warp per body up to this many bodies (B2D_BP_WARP_MAX)
     void *cub_tmp = nullptr; size_t cub_tmp_bytes = 0;
@@ -235,6 +235,8 @@ b2d_world *b2d_create(const b2d_config *cfg) {
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_solve_tiles, TILE_CAP, TILE_SOLVE_SMEM); w->tile_blocks = std::max(1, per_sm) * w->num_sms;
     cudaFuncSetAttribute(k_island_tiles, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TILE_FUSED_SMEM);
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_island_tiles, TILE_CAP, TILE_FUSED_SMEM); w->tile_fused_blocks = std::max(1, per_sm) * w->num_sms;
+    cudaFuncSetAttribute(k_island_tiles_2p, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TILE_FUSED_SMEM_2P);
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_island_tiles_2p, TILE_CAP, TILE_FUSED_SMEM_2P); w->tile_fused_blocks_2p = std::max(1, per_sm) * w->num_sms;
     if (const char *e = getenv("B2D_BP_WARP_MAX")) w->bp_warp_max = (uint32_t)std::max(0, atoi(e));
     if (const char *e = getenv("B2D_TILES")) if (atoi(e) == 0) d.max_tiles = 0;          // development: everything through the dataflow path
     if (const char *e = getenv("B2D_GRAPH")) w->use_graph = atoi(e) != 0;
@@ -682,7 +684,10 @@ static int enqueue_solver_b(b2d_world *w) {
     const int pi = (int)w->cfg.position_iterations;
     if (d.max_tiles) {
         // with position iterations: the tiled islands' whole solver.update in one launch; without: the velocity part alone
-        if (pi > 0) { k_island_tiles<<<w->tile_fused_blocks, TILE_CAP, TILE_FUSED_SMEM, w->stream>>>(d, vi, pi); ++w->launches; }
+        if (pi > 0) {       // two-point tiles [0, ntiles2), then the generic ones
+            k_island_tiles_2p<<<w->tile_fused_blocks_2p, TILE_CAP, TILE_FUSED_SMEM_2P, w->stream>>>(d, vi, pi); ++w->launches;
+            k_island_tiles<<<w->tile_fused_blocks, TILE_CAP, TILE_FUSED_SMEM, w->stream>>>(d, vi, pi); ++w->launches;
+        }
         else { k_solve_tiles<<<w->tile_blocks, TILE_CAP, TILE_SOLVE_SMEM, w->stream>>>(d, vi); ++w->launches; }
     }
     CK(coop_launch(w, k_solve_df, w->coop_blocks_df, B2D_SOLVE_THREADS, d, vi));

@@ -650,9 +650,13 @@ __global__ void __launch_bounds__(128) k_np_merge(Dev d) {
         for (int s = 0; s < num; ++s) store_point(d, m, s, P[s]);
         d.mstate[m] = (st & ~MS_NPTS_MASK) | (uint32_t)num;
         // the island rebuild reads whether a manifold has points (colouring, island census) and, on the dataflow path,
-        // its point count (sort key); inside an island tile the count only matters to the solver itself
+        // its point count (sort key); inside an island tile the count only matters to the solver itself, except that a
+        // two-point tile has no room for a third point
         const uint32_t was = st & MS_NPTS_MASK;
-        if ((uint32_t)num != was && (was == 0u || num == 0 || d.btile[key_body(d, pr)] == TILE_NONE)) d.cnt->graph_changed = 1u;
+        if ((uint32_t)num != was) {
+            const uint32_t tile = d.btile[key_body(d, pr)];
+            if (was == 0u || num == 0 || tile == TILE_NONE || (num > 2 && was <= 2u && tile < d.cnt->ntiles2)) d.cnt->graph_changed = 1u;
+        }
     }
 }
 
@@ -838,7 +842,12 @@ __global__ void k_color_list(Dev d, int recolor) {
             if (da) atomicOr(&d.bmask[p.x], 1ULL << col);
             if (db) atomicOr(&d.bmask[p.y], 1ULL << col);
         }
-        island_count(d.isl_nm, d.parent[da ? p.x : p.y]);
+        const uint32_t root = d.parent[da ? p.x : p.y];
+        island_count(d.isl_nm, root);
+        {   // one atomic per island per warp, as in island_count (a pile of boxes is one island)
+            const uint32_t grp = __match_any_sync(__activemask(), root), multi = __ballot_sync(__activemask(), (st & MS_NPTS_MASK) > 2u);
+            if ((grp & multi) && (threadIdx.x & 31u) == (uint32_t)(__ffs(grp) - 1)) atomicOr(&d.isl_nm[root], ISL_MULTIPOINT);
+        }
     }
     GRID_STRIDE(h, d.nhinges) {
         uint2 p = d.hpair[h];
@@ -906,15 +915,20 @@ __global__ void __launch_bounds__(256) k_color(Dev d) {
 // w = max(bodies, manifolds, joints) <= TILE_ISLAND_MAX per island and P the exclusive prefix sum of the weights, island
 // -> tile P / g with g = TILE_CAP + 1 - (heaviest tiled island) puts at most TILE_CAP of each into every tile.  Which islands
 // are tiled changes speed, never results: the per-body constraint order is fixed by the colours alone.
+// Two classes, each packed this way in root order: two-point islands (no manifold with more than 2 points: spheres,
+// capsules, planes) in tiles [0, ntiles2), solved by the two-point kernel, then the others in [ntiles2, ntiles).  The
+// two prefix sums are the two words of one 64-bit scan.
 __global__ void k_tile_weights(Dev d) {
     uint32_t wmax = 0;
     GRID_STRIDE(i, d.nbodies) {
         uint32_t w = 0;
+        bool multi = false;
         if (is_dynamic(d.flags[i]) && d.parent[i] == i) {
-            const uint32_t nb = d.isl_nb[i], nm = d.isl_nm[i], nh = d.isl_nh[i];
+            const uint32_t nb = d.isl_nb[i], nm = d.isl_nm[i] & ~ISL_MULTIPOINT, nh = d.isl_nh[i];
+            multi = (d.isl_nm[i] & ISL_MULTIPOINT) != 0u;
             if (nb <= TILE_ISLAND_MAX && nm <= TILE_ISLAND_MAX && nh <= TILE_ISLAND_MAX && (nm | nh)) w = max(nb, max(nm, nh));
         }
-        d.swgt[i] = w;
+        d.swgt[i] = multi ? (unsigned long long)w << 32 : w;
         wmax = max(wmax, w);
     }
     wmax = __reduce_max_sync(0xffffffffu, wmax);
@@ -924,13 +938,19 @@ __global__ void k_tile_weights(Dev d) {
 B2D_D uint32_t tile_granule(const Dev &d) { return (uint32_t)TILE_CAP + 1u - max(d.cnt->tile_wmax, 1u); }
 __global__ void k_tile_assign(Dev d) {
     const uint32_t n = d.nbodies, g = tile_granule(d);
-    if (blockIdx.x == 0 && threadIdx.x == 0) d.cnt->ntiles = min(d.max_tiles, (d.swsum[n - 1] + d.swgt[n - 1] + g - 1) / g);
+    const unsigned long long total = d.swsum[n - 1] + d.swgt[n - 1];
+    const uint32_t ntiles2 = ((uint32_t)total + g - 1) / g;
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        d.cnt->ntiles2 = min(d.max_tiles, ntiles2);
+        d.cnt->ntiles = min(d.max_tiles, ntiles2 + ((uint32_t)(total >> 32) + g - 1) / g);
+    }
     GRID_STRIDE(i, n) {
         uint32_t tile = TILE_NONE, slot = SLOT_NONE;
         if (is_dynamic(d.flags[i])) {
             const uint32_t r = d.parent[i];
             if (d.swgt[r]) {
-                tile = d.swsum[r] / g;
+                const unsigned long long p = d.swsum[r];
+                tile = (d.swgt[r] >> 32) ? ntiles2 + (uint32_t)(p >> 32) / g : (uint32_t)p / g;
                 if (tile < d.max_tiles) {                           // order within the tile is immaterial; one atomic per tile per warp
                     const uint32_t grp = __match_any_sync(__activemask(), tile), lane = threadIdx.x & 31u, leader = (uint32_t)(__ffs(grp) - 1);
                     uint32_t base = 0;
@@ -1709,10 +1729,19 @@ B2D_D void tile_error_max(uint32_t *s_err, uint32_t islot, float err) { if (err 
 // where they sit (shared memory), the impulses go straight to the warm-start cache, the position iterations run on
 // the same records, and positions / orientations / velocities are written once.  Same arithmetic in the same order as
 // the separate kernels (k_prepare_contacts, k_prepare_hinges, k_integrate, k_store_impulses skip what this kernel has done).
-// shared memory of a tile, float4 x TILE_CAP each: body records [0..7] -- row preparation: linvel, angvel, inv_IW rows
-// (| inv_m), pos, orn; velocity phase: dv, dw, inv_IW rows; position phase: pos | inv_m, orn, inv_IW rows, inv_I rows --,
-// joint rows [8..14], contact points 3-4 [15..24] (solver rows, then pA pB pN pL)
+// Two specialisations of one body (island_tiles<MAXP>), by the most contact points a manifold of the tile may have:
+// k_island_tiles (4) for the generic tiles, k_island_tiles_2p (2) for the two-point tiles, which keep less in registers
+// (ptxas: 40 B of spills at the 128-register cap instead of 280 B; under a 3-CTA bound, 80 registers, it spilled 646 B and
+// ran slower than the generic kernel on chains_1048576).  Shared memory of a tile, float4 x TILE_CAP each: body records [0..7] -- row preparation: linvel,
+// angvel, inv_IW rows (| inv_m), pos, orn; velocity phase: dv, dw, inv_IW rows; position phase: pos | inv_m, orn, inv_IW
+// rows, inv_I rows --, then
+//   generic:   joint rows [8..14], contact points 3-4 [15..24] (solver rows, then pA pB pN pL); the solver rows of points
+//              1-2 and the position-phase data of points 1-2 in registers;
+//   two-point: joint rows [10..16], the solver rows of point 2 in [5..9] during the velocity iterations (body records
+//              5-7 are idle then), pA pB pN pL of points 1-2 in [8..15] during the position iterations (the joint rows
+//              are dead then); only the solver rows of point 1 in registers.
 constexpr size_t TILE_FUSED_SMEM = (8 + 7 + 10) * TILE_CAP * sizeof(float4);
+constexpr size_t TILE_FUSED_SMEM_2P = (8 + 2 + 7) * TILE_CAP * sizeof(float4);
 // solver_body (+ position, orientation, record slot) of body `id` of a tiled constraint during the row preparation: a
 // dynamic body from the records staged by slot, a static / kinematic one from global memory
 B2D_D void tile_solver_body(const Dev &d, const float4 *sb, uint32_t id, SBody &s, v3 &pos, q4 &orn, uint32_t &slot) {
@@ -1750,14 +1779,17 @@ B2D_D void tq_store(float4 *sb, uint32_t slot, const PBody &b) {
     sb[slot] = f4(b.pos, b.inv_m); sb[TILE_CAP + slot] = f4(b.orn);
     sb[2 * TILE_CAP + slot] = f4(b.inv_IW.r0, 0); sb[3 * TILE_CAP + slot] = f4(b.inv_IW.r1, 0); sb[4 * TILE_CAP + slot] = f4(b.inv_IW.r2, 0);
 }
-__global__ void __launch_bounds__(TILE_CAP, 2) k_island_tiles(Dev d, int vel_iters, int pos_iters) {
+template <int MAXP>
+B2D_D void island_tiles(const Dev &d, int vel_iters, int pos_iters) {
+    constexpr bool TWO = MAXP == 2;
     extern __shared__ float4 s_tile[];
-    float4 *s_body = s_tile, *s_hr = s_tile + 8 * TILE_CAP, *s_row = s_tile + 15 * TILE_CAP;
+    float4 *s_body = s_tile, *s_hr = s_tile + (TWO ? 10 : 8) * TILE_CAP, *s_row = s_tile + 15 * TILE_CAP;
+    float4 *s_p2 = s_tile + 5 * TILE_CAP + threadIdx.x, *s_pt = s_tile + 8 * TILE_CAP + threadIdx.x;       // two-point only
     __shared__ uint32_t s_err[TILE_CAP], s_done[TILE_CAP], s_root[TILE_CAP];
     __shared__ uint32_t s_ncol[2];
-    const uint32_t ntiles = d.cnt->ntiles, t = threadIdx.x;
+    const uint32_t tile0 = TWO ? 0u : d.cnt->ntiles2, ntiles = TWO ? d.cnt->ntiles2 : d.cnt->ntiles, t = threadIdx.x;
     const size_t NM = d.NM;
-    for (uint32_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    for (uint32_t tile = tile0 + blockIdx.x; tile < ntiles; tile += gridDim.x) {
         const uint32_t nb = min(d.tile_nb[tile], (uint32_t)TILE_CAP);
         const uint32_t c0 = d.tile_c0[tile], c1 = min(d.tile_c1[tile], c0 + TILE_CAP), h0 = d.tile_h0[tile], h1 = min(d.tile_h1[tile], h0 + TILE_CAP);
         if (t < 2) s_ncol[t] = 0;
@@ -1794,10 +1826,12 @@ __global__ void __launch_bounds__(TILE_CAP, 2) k_island_tiles(Dev d, int vel_ite
             const uint32_t npts = d.mstate[m] & MS_NPTS_MASK;
             SBody A, B; v3 posA, posB; q4 ornA, ornB; uint32_t sa, sb;
             tile_solver_body(d, s_body, pr.x, A, posA, ornA, sa); tile_solver_body(d, s_body, pr.y, B, posB, ornB, sb);
-            ch = make_uint4(pr.x | (A.proc ? 0u : 0x80000000u), pr.y | (B.proc ? 0u : 0x80000000u), npts, sa | (sb << 16));
+            // a two-point tile holds no manifold with more points: one that gains a third point sets graph_changed
+            // (k_np_merge) and the rebuild moves its island to a generic tile before the next solve
+            ch = make_uint4(pr.x | (A.proc ? 0u : 0x80000000u), pr.y | (B.proc ? 0u : 0x80000000u), TWO ? min(npts, 2u) : npts, sa | (sb << 16));
             contact_point_rows(d, m, A, B, posA, ornA, posB, ornB, a0, a1, a2, a3, aim);
             if (npts > 1) contact_point_rows(d, NM + m, A, B, posA, ornA, posB, ornB, b0, b1, b2, b3, bim);
-            for (uint32_t s = 2; s < npts; ++s) {
+            if (!TWO) for (uint32_t s = 2; s < npts; ++s) {
                 float4 *r = s_row + (s - 2) * 5 * TILE_CAP + t;
                 contact_point_rows(d, s * NM + m, A, B, posA, ornA, posB, ornB, r[0], r[TILE_CAP], r[2 * TILE_CAP], r[3 * TILE_CAP], r[4 * TILE_CAP]);
             }
@@ -1806,6 +1840,7 @@ __global__ void __launch_bounds__(TILE_CAP, 2) k_island_tiles(Dev d, int vel_ite
         }
         __syncthreads();
         if (t < nb) { s_body[t] = make_float4(0, 0, 0, 0); s_body[TILE_CAP + t] = make_float4(0, 0, 0, 0); }
+        if (TWO && ch.z > 1) { s_p2[0] = b0; s_p2[TILE_CAP] = b1; s_p2[2 * TILE_CAP] = b2; s_p2[3 * TILE_CAP] = b3; s_p2[4 * TILE_CAP] = bim; }
         __syncthreads();
         const uint32_t nhc = s_ncol[0], ncc = s_ncol[1];
         // ---- velocity iterations (as in k_solve_tiles)
@@ -1828,8 +1863,13 @@ __global__ void __launch_bounds__(TILE_CAP, 2) k_island_tiles(Dev d, int vel_ite
                 if (ccol == c) {
                     VBody A, B; tf_load(s_body, ch.x, ch.w & 0xFFFFu, A); tf_load(s_body, ch.y, ch.w >> 16, B);
                     nrow_solve(a0, a1, a2, aim, A, B, warm);
-                    if (ch.z > 1) nrow_solve(b0, b1, b2, bim, A, B, warm);
-                    for (uint32_t s = 2; s < ch.z; ++s) {
+                    if (TWO && ch.z > 1) {
+                        float4 im = s_p2[4 * TILE_CAP];
+                        nrow_solve(s_p2[0], s_p2[TILE_CAP], s_p2[2 * TILE_CAP], im, A, B, warm);
+                        s_p2[4 * TILE_CAP] = im;
+                    }
+                    if (!TWO && ch.z > 1) nrow_solve(b0, b1, b2, bim, A, B, warm);
+                    if (!TWO) for (uint32_t s = 2; s < ch.z; ++s) {
                         float4 *r = s_row + (s - 2) * 5 * TILE_CAP + t;
                         float4 im = r[4 * TILE_CAP];
                         nrow_solve(r[0], r[TILE_CAP], r[2 * TILE_CAP], im, A, B, warm);
@@ -1843,8 +1883,13 @@ __global__ void __launch_bounds__(TILE_CAP, 2) k_island_tiles(Dev d, int vel_ite
                 if (ccol == c) {
                     VBody A, B; tf_load(s_body, ch.x, ch.w & 0xFFFFu, A); tf_load(s_body, ch.y, ch.w >> 16, B);
                     frow_solve(a0, a1, a2, a3, aim, A, B, warm);
-                    if (ch.z > 1) frow_solve(b0, b1, b2, b3, bim, A, B, warm);
-                    for (uint32_t s = 2; s < ch.z; ++s) {
+                    if (TWO && ch.z > 1) {
+                        float4 im = s_p2[4 * TILE_CAP];
+                        frow_solve(s_p2[0], s_p2[TILE_CAP], s_p2[2 * TILE_CAP], s_p2[3 * TILE_CAP], im, A, B, warm);
+                        s_p2[4 * TILE_CAP] = im;
+                    }
+                    if (!TWO && ch.z > 1) frow_solve(b0, b1, b2, b3, bim, A, B, warm);
+                    if (!TWO) for (uint32_t s = 2; s < ch.z; ++s) {
                         float4 *r = s_row + (s - 2) * 5 * TILE_CAP + t;
                         float4 im = r[4 * TILE_CAP];
                         frow_solve(r[0], r[TILE_CAP], r[2 * TILE_CAP], r[3 * TILE_CAP], im, A, B, warm);
@@ -1859,8 +1904,8 @@ __global__ void __launch_bounds__(TILE_CAP, 2) k_island_tiles(Dev d, int vel_ite
         uint32_t m = 0;
         if (hasC) {
             m = d.cidx_s[ci];
-            d.pI[m] = aim; if (ch.z > 1) d.pI[NM + m] = bim;
-            for (uint32_t s = 2; s < ch.z; ++s) d.pI[s * NM + m] = s_row[((s - 2) * 5 + 4) * TILE_CAP + t];
+            d.pI[m] = aim; if (ch.z > 1) d.pI[NM + m] = TWO ? s_p2[4 * TILE_CAP] : bim;
+            if (!TWO) for (uint32_t s = 2; s < ch.z; ++s) d.pI[s * NM + m] = s_row[((s - 2) * 5 + 4) * TILE_CAP + t];
         }
         if (hasH) {
             const float4 r5 = s_hr[5 * TILE_CAP + t], r6 = s_hr[6 * TILE_CAP + t];
@@ -1880,16 +1925,18 @@ __global__ void __launch_bounds__(TILE_CAP, 2) k_island_tiles(Dev d, int vel_ite
         }
         if (hasC) {
             cisl = d.bslot[island_of(d, ch.x & 0x7FFFFFFFu, ch.y & 0x7FFFFFFFu)];
-            a40 = d.pA[m]; b40 = d.pB[m]; n40 = d.pN[m]; l40 = d.pL[m];
-            if (ch.z > 1) { a41 = d.pA[NM + m]; b41 = d.pB[NM + m]; n41 = d.pN[NM + m]; l41 = d.pL[NM + m]; }
+            if (!TWO) {
+                a40 = d.pA[m]; b40 = d.pB[m]; n40 = d.pN[m]; l40 = d.pL[m];
+                if (ch.z > 1) { a41 = d.pA[NM + m]; b41 = d.pB[NM + m]; n41 = d.pN[NM + m]; l41 = d.pL[NM + m]; }
+            }
         }
         float4 hpos = spos, horn = sorn;                        // a joint to a static / kinematic body
         if (hasC && ((ch.x | ch.y) >> 31)) { const uint32_t sbody = ((ch.x >> 31) ? ch.x : ch.y) & 0x7FFFFFFFu; spos = d.pos[sbody]; sorn = d.orn[sbody]; }
         if (hasH && ((hh.x | hh.y) >> 31)) { const uint32_t sbody = ((hh.x >> 31) ? hh.x : hh.y) & 0x7FFFFFFFu; hpos = d.pos[sbody]; horn = d.orn[sbody]; }
-        __syncthreads();                                         // the rows in s_row are dead from here on
-        if (hasC) for (uint32_t s = 2; s < ch.z; ++s) {
+        __syncthreads();                                         // the rows in s_row (two-point: s_p2, s_hr) are dead from here on
+        if (hasC) for (uint32_t s = TWO ? 0 : 2; s < ch.z; ++s) {
             const size_t mi = s * NM + m;
-            float4 *r = s_row + (s - 2) * 4 * TILE_CAP + t;
+            float4 *r = TWO ? s_pt + s * 4 * TILE_CAP : s_row + (s - 2) * 4 * TILE_CAP + t;
             r[0] = d.pA[mi]; r[TILE_CAP] = d.pB[mi]; r[2 * TILE_CAP] = d.pN[mi]; r[3 * TILE_CAP] = d.pL[mi];
         }
         // ---- integrate_velocities (k_integrate) for the tile's bodies; the records turn into position records
@@ -1947,10 +1994,12 @@ __global__ void __launch_bounds__(TILE_CAP, 2) k_island_tiles(Dev d, int vel_ite
                         if (dist > -EPS) return;
                         position_solve(A, B, normal, cross(rA, normal), -normal, -cross(rB, normal), -dist, max_error);
                     };
-                    point(a40, b40, n40, l40);
-                    if (ch.z > 1) point(a41, b41, n41, l41);
-                    for (uint32_t s = 2; s < ch.z; ++s) {
-                        float4 *r = s_row + (s - 2) * 4 * TILE_CAP + t;
+                    if (!TWO) {
+                        point(a40, b40, n40, l40);
+                        if (ch.z > 1) point(a41, b41, n41, l41);
+                    }
+                    for (uint32_t s = TWO ? 0 : 2; s < ch.z; ++s) {
+                        float4 *r = TWO ? s_pt + s * 4 * TILE_CAP : s_row + (s - 2) * 4 * TILE_CAP + t;
                         float4 pa = r[0], pn = r[2 * TILE_CAP];
                         point(pa, r[TILE_CAP], pn, r[3 * TILE_CAP]);
                         r[0] = pa; r[2 * TILE_CAP] = pn;
@@ -1966,9 +2015,14 @@ __global__ void __launch_bounds__(TILE_CAP, 2) k_island_tiles(Dev d, int vel_ite
             }
         }
         if (hasC) {
-            d.pN[m] = n40; d.pA[m] = a40;
-            if (ch.z > 1) { d.pN[NM + m] = n41; d.pA[NM + m] = a41; }
-            for (uint32_t s = 2; s < ch.z; ++s) { const float4 *r = s_row + (s - 2) * 4 * TILE_CAP + t; d.pA[s * NM + m] = r[0]; d.pN[s * NM + m] = r[2 * TILE_CAP]; }
+            if (!TWO) {
+                d.pN[m] = n40; d.pA[m] = a40;
+                if (ch.z > 1) { d.pN[NM + m] = n41; d.pA[NM + m] = a41; }
+            }
+            for (uint32_t s = TWO ? 0 : 2; s < ch.z; ++s) {
+                const float4 *r = TWO ? s_pt + s * 4 * TILE_CAP : s_row + (s - 2) * 4 * TILE_CAP + t;
+                d.pA[s * NM + m] = r[0]; d.pN[s * NM + m] = r[2 * TILE_CAP];
+            }
         }
         if (t < nb) {
             const float4 p = s_body[t];
@@ -1977,6 +2031,9 @@ __global__ void __launch_bounds__(TILE_CAP, 2) k_island_tiles(Dev d, int vel_ite
         __syncthreads();
     }
 }
+
+__global__ void __launch_bounds__(TILE_CAP, 2) k_island_tiles(Dev d, int vel_iters, int pos_iters) { island_tiles<4>(d, vel_iters, pos_iters); }
+__global__ void __launch_bounds__(TILE_CAP, 2) k_island_tiles_2p(Dev d, int vel_iters, int pos_iters) { island_tiles<2>(d, vel_iters, pos_iters); }
 
 // ---------------------------------------------------------------------- dataflow: position iterations
 #ifndef B2D_POS_MIN_BLOCKS

@@ -33,6 +33,7 @@ constexpr int MAX_COLORS = 64;
 constexpr int TILE_CAP = B2D_TILE_CAP;         // threads per tile CTA = capacity in bodies, manifolds and joints
 constexpr int TILE_ISLAND_MAX = TILE_CAP / 2;  // an island is tiled if it has at most this many bodies, manifolds and joints
 constexpr uint32_t TILE_NONE = 0xFFFFFFFFu;
+constexpr uint32_t ISL_MULTIPOINT = 0x80000000u;  // isl_nm flag: a manifold of the island has more than 2 points
 constexpr uint32_t SLOT_NONE = 0xFFFFu;
 // sort keys.  tiled: tile(16) | colour(6); dataflow: DF | colour(6) | points-1 (2) | spatial rank(14); no rows: INACTIVE
 constexpr int KEY_TILE_BITS = 16;                                   // 24-bit keys: three radix passes
@@ -66,6 +67,7 @@ struct Counters {
     uint32_t speed;          // float bits: fastest point of any dynamic body, m/s (multi-GPU exchange)
     uint32_t nhactive;               // hinges with rows this step
     uint32_t ntiles;                 // island tiles this step
+    uint32_t ntiles2;                // of which two-point tiles: [0, ntiles2); generic tiles [ntiles2, ntiles)
     uint32_t tile_wmax;              // heaviest tiled island (zeroed by the host, like the next two)
     uint32_t ncolors_all, nhcolors_all;      // colours in use over both solver paths (statistics)
     uint32_t ntiled, nhtiled;        // contact manifolds / hinges solved in tiles: [0, ntiled) of the sorted arrays
@@ -111,8 +113,9 @@ struct Dev {
     uint32_t *brank;                     // position of every body in the sorted cell order (spatial rank)
     // ---- island tiles
     uint32_t max_tiles;
-    uint32_t *isl_nb, *isl_nm, *isl_nh;  // per island root: dynamic bodies, manifolds with points, joints
-    uint32_t *swgt, *swsum;              // per body id: packing weight of the island it is the root of, exclusive prefix sum
+    uint32_t *isl_nb, *isl_nm, *isl_nh;  // per island root: dynamic bodies, manifolds with points (| ISL_MULTIPOINT), joints
+    unsigned long long *swgt, *swsum;    // per body id: packing weight of the island it is the root of (two-point islands in
+                                         // the low word, the others in the high word), exclusive prefix sum
     uint32_t *btile, *bslot;             // per body: tile of its island (TILE_NONE: dataflow path), record slot in the tile
     uint32_t *tile_nb, *tile_body;       // per tile: bodies, slot -> body (TILE_CAP per tile)
     uint32_t *tile_c0, *tile_c1, *tile_h0, *tile_h1;   // per tile: its range of the sorted contact / hinge arrays
