@@ -1170,6 +1170,31 @@ int b2d_debug_tiles(b2d_world *w, uint32_t *out6) {
     out6[5] = nb.empty() ? 0u : *std::max_element(nb.begin(), nb.end());
     return B2D_OK;
 }
+// development aid: the island-tile packing of the last rebuild, as the solve reads it (include/b2d.h)
+int b2d_debug_tile_map(b2d_world *w, uint32_t *counts5, uint32_t *btile, uint32_t *bslot, uint32_t *tiles5,
+                       uint32_t *tiled_pairs, uint32_t *tiled_hinges) {
+    if (!w || !counts5) return B2D_ERR_ARGUMENT;
+    cudaSetDevice(w->cfg.device);
+    const Dev &d = w->d;
+    Counters c; int rc = fetch_counters(w, c); if (rc) return rc;
+    const uint32_t nt = std::min(c.ntiles, d.max_tiles), ntc = std::min(c.ntiled, d.NM), nth = std::min(c.nhtiled, d.NH);
+    counts5[0] = nt; counts5[1] = std::min(c.ntiles2, nt); counts5[2] = ntc; counts5[3] = nth; counts5[4] = d.max_tiles;
+    if (btile && d.nbodies) CK(cudaMemcpy(btile, d.btile, d.nbodies * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    if (bslot && d.nbodies) CK(cudaMemcpy(bslot, d.bslot, d.nbodies * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    if (tiles5 && nt) {
+        const uint32_t *src[5] = {d.tile_nb, d.tile_c0, d.tile_c1, d.tile_h0, d.tile_h1};
+        for (int k = 0; k < 5; ++k) CK(cudaMemcpy(tiles5 + (size_t)k * nt, src[k], nt * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    }
+    if (tiled_pairs && ntc) {
+        std::vector<uint32_t> ci(ntc);
+        std::vector<uint2> mp(d.NM);
+        CK(cudaMemcpy(ci.data(), d.cidx_s, ntc * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(mp.data(), d.mpair, d.NM * sizeof(uint2), cudaMemcpyDeviceToHost));
+        for (uint32_t i = 0; i < ntc; ++i) { tiled_pairs[2 * i] = mp[ci[i]].x; tiled_pairs[2 * i + 1] = mp[ci[i]].y; }
+    }
+    if (tiled_hinges && nth) CK(cudaMemcpy(tiled_hinges, d.hidx_s, nth * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    return B2D_OK;
+}
 int b2d_reset_timers(b2d_world *w) { if (!w) return B2D_ERR_ARGUMENT; w->timed_steps = 0; return B2D_OK; }
 
 int b2d_set_halo_margin(b2d_world *w, float margin) {

@@ -346,6 +346,22 @@ class World:
         self._check(self.l.b2d_debug_tiles(self.h, _p(out)))
         return dict(zip(("tiles", "tiled_manifolds", "tiled_hinges", "active_manifolds", "active_hinges", "max_bodies_per_tile"), out.tolist()))
 
+    def debug_tile_map(self):
+        """Development aid: the island-tile packing of the last rebuild (b2d_debug_tile_map).  Per body its tile and record
+        slot (0xFFFFFFFF / 0xFFFF: not tiled); per tile its body count and its [c0, c1) / [h0, h1) ranges into
+        `pairs` (the body pairs of the tiled manifolds) and `hinges` (the tiled hinge ids)."""
+        cnt = np.zeros(5, u32)
+        self._check(self.l.b2d_debug_tile_map(self.h, _p(cnt), None, None, None, None, None))
+        nt, nt2, nc, nh, cap = (int(x) for x in cnt)
+        n = max(1, self.cfg.max_bodies)
+        btile, bslot = np.zeros(n, u32), np.zeros(n, u32)
+        tiles, pairs, hinges = np.zeros((5, max(1, nt)), u32), np.zeros((max(1, nc), 2), u32), np.zeros(max(1, nh), u32)
+        self._check(self.l.b2d_debug_tile_map(self.h, _p(cnt), _p(btile), _p(bslot), _p(tiles), _p(pairs), _p(hinges)))
+        return dict(ntiles=nt, ntiles2=nt2, ntiled=nc, nhtiled=nh, max_tiles=cap, btile=btile[:self.num_bodies],
+                    bslot=bslot[:self.num_bodies], tile_nb=tiles[0, :nt].copy(), tile_c0=tiles[1, :nt].copy(),
+                    tile_c1=tiles[2, :nt].copy(), tile_h0=tiles[3, :nt].copy(), tile_h1=tiles[4, :nt].copy(),
+                    pairs=pairs[:nc], hinges=hinges[:nh])
+
     def stats(self) -> dict:
         s = Stats()
         self._check(self.l.b2d_get_stats(self.h, C.byref(s)))

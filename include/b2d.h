@@ -195,6 +195,15 @@ int b2d_debug_counters(b2d_world *w, void *out, uint32_t bytes);
 /* Development aid: the island tiles of the last step (DESIGN.md section 2): out6 = tiles, manifolds / hinges solved in
  * tiles, manifolds / hinges with rows, most bodies in one tile. */
 int b2d_debug_tiles(b2d_world *w, uint32_t *out6);
+/* Development aid: the island-tile packing of the last island rebuild, which later steps reuse while the constraint graph
+ * is unchanged.  counts5 = tiles (two-point tiles first), two-point tiles, manifolds / hinges solved in tiles, tile
+ * capacity of the world.  Each of the other outputs may be NULL: btile / bslot (one word per body: its tile and record
+ * slot, 0xFFFFFFFF / 0xFFFF when it is not in a tile), tiles5 (5 x tiles words, row-major: bodies, then the
+ * [c0, c1) and [h0, h1) ranges into the tiled constraints), tiled_pairs (2 x manifolds in tiles: the body pairs of the
+ * tiled manifolds in that order), tiled_hinges (hinges in tiles: hinge ids in that order).  Call with NULLs first for
+ * the sizes. */
+int b2d_debug_tile_map(b2d_world *w, uint32_t *counts5, uint32_t *btile, uint32_t *bslot, uint32_t *tiles5,
+                       uint32_t *tiled_pairs, uint32_t *tiled_hinges);
 /* Multi-GPU exchange (SURVEY.md section 8e): enqueue, on the world's stream, the reduction of all dynamic AABBs into
  * device_out8 = {min xyz, max xyz, speed, 0} -- a DEVICE pointer (e.g. a buffer owned by the host framework) the adapter
  * then all-gathers over NCCL to detect island groups of different ranks coming within the broadphase margin of each

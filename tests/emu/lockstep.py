@@ -1,7 +1,8 @@
 """TEST INFRASTRUCTURE.  The library's CUDA kernels, executed by the CPU emulation (tests/emu), in lock step with the
 oracle through the normal Python adapter and C ABI -- the same comparison tests/test_gpu_parity.py makes on the GPU: ordered
 pair lists identical, post-solve state within 1e-5 (here: identical, glibc's sinf / cosf on both sides) with the oracle
-replaying the device's Gauss-Seidel order, manifolds and joint impulses re-synchronised every step.
+replaying the device's Gauss-Seidel order, manifolds and joint impulses re-synchronised every step.  The -m gpu lock-step
+tests (test_gpu_tile_edges.py, test_gpu_random_lockstep.py) call `lockstep` in-process, on the GPU or the emulation.
 
     python tests/emu/lockstep.py fixed|narrow|wide FIRST LAST [--tiles 0|1] [--steps N] [--restitution] [--mutate]     -> one JSON line
 Runs in its own process because B2D_LIB has to be set before edyn_b200 is imported."""
@@ -15,10 +16,43 @@ ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
 
 
-def lockstep(E, O, scene, steps, restitution_solver=False):
+# How the device runs the step: plain launches that rebuild the islands every step, CUDA graphs that skip the rebuild while
+# the constraint graph is unchanged, and everything on the dataflow path (no island tiles).  The emulation launches plainly.
+MODES = {"plain": dict(B2D_GRAPH="0", B2D_GRAPH_REUSE="1", B2D_TILES="1"),
+         "graph": dict(B2D_GRAPH="1", B2D_GRAPH_REUSE="1", B2D_TILES="1"),
+         "dataflow": dict(B2D_GRAPH="0", B2D_GRAPH_REUSE="1", B2D_TILES="0")}
+STATE_KEYS = ("pos", "orn", "linvel", "angvel", "aabb")
+
+
+def build_world(E, scene, mode=None, **kw):
+    """E.scenes.build_world with the environment of `mode` (read when the world is created); None: as the environment is."""
+    if mode is None:
+        return E.scenes.build_world(scene, **kw)
+    saved = {k: os.environ.get(k) for k in MODES[mode]}
+    os.environ.update(MODES[mode])
+    try:
+        return E.scenes.build_world(scene, **kw)
+    finally:
+        for k, v in saved.items():
+            if v is None:
+                os.environ.pop(k, None)
+            else:
+                os.environ[k] = v
+
+
+def lockstep(E, O, scene, steps, restitution_solver=False, mode=None, hook=None, vel_iters=None, pos_iters=None):
+    """One device world in `mode` (a key of MODES; None: as the environment says) against the oracle, `steps` single
+    steps.  vel_iters / pos_iters override the scene's settings on both sides; hook(step, world) runs after each step's comparison (and may assert).  Returns ok, worst
+    (largest state difference), exact (bit-identical steps), points (contact points at the end), max_points (most points
+    in one manifold at any step), flags, and digests: one hash of the device state per step, for comparing modes."""
+    import hashlib
     import numpy as np
-    w = E.scenes.build_world(scene, flags=E.world.FLAG_RESTITUTION_SOLVER if restitution_solver else 0)
-    st = scene["settings"]
+    st = dict(scene["settings"])
+    if vel_iters is not None:
+        st["velocity_iterations"] = vel_iters
+    if pos_iters is not None:
+        st["position_iterations"] = pos_iters
+    w = build_world(E, scene, mode, flags=E.world.FLAG_RESTITUTION_SOLVER if restitution_solver else 0, **st)
     o = O.OracleWorld(vel_iters=st["velocity_iterations"], pos_iters=st["position_iterations"])
     if restitution_solver:
         o.set_restitution_iterations(8, 3)          # no graph order handed over: the oracle's defaults are the device's conventions
@@ -28,7 +62,7 @@ def lockstep(E, O, scene, steps, restitution_solver=False):
         o.add_hinges(h["a"], h["b"], h["pivot_a"], h["pivot_b"], h["axis_a"], h["axis_b"])
     if scene["exclusions"] is not None:
         o.add_exclusions(*scene["exclusions"])
-    worst = 0.0
+    worst, exact, max_points, digests = 0.0, 0, 0, []
     for s in range(steps):
         w.step(1)
         hi, pr = w.solver_order()
@@ -40,18 +74,24 @@ def lockstep(E, O, scene, steps, restitution_solver=False):
             return dict(ok=False, step=s, why="ordered broadphase pair lists differ")
         if not np.array_equal(w.islands(), o.islands()):
             return dict(ok=False, step=s, why="island labels differ")
-        err = max(float(np.abs(g[k] - c[k]).max()) for k in ("pos", "orn", "linvel", "angvel", "aabb"))
+        err = max(float(np.abs(g[k] - c[k]).max()) for k in STATE_KEYS)
         worst = max(worst, err)
+        exact += err == 0.0
         if err > 1e-5:
             return dict(ok=False, step=s, why=f"state differs by {err:.3e}")
+        digests.append(hashlib.sha1(b"".join(np.ascontiguousarray(g[k]).tobytes() for k in STATE_KEYS)).hexdigest())
         o.set_state(g["pos"], g["orn"], g["linvel"], g["angvel"])
         gc = w.contacts()
+        max_points = max(max_points, int(gc["num"].max(initial=0)))
         o.set_contacts(gc["pairs"], gc["num"], gc["pts"], gc["att"], gc["lifetime"])
         if scene["hinges"]:
             o.set_hinge_impulses(w.hinge_impulses())
+        if hook is not None:
+            hook(s, w)
     stats = w.stats()
     w.close()
-    return dict(ok=stats["error_flags"] == 0, worst=worst, points=int(stats["contact_points"]), flags=int(stats["error_flags"]))
+    return dict(ok=stats["error_flags"] == 0, worst=worst, exact=exact, points=int(stats["contact_points"]), max_points=max_points,
+                flags=int(stats["error_flags"]), reused=int(stats["steps_reused"]), digests=digests)
 
 
 def lockstep_with_mutations(E, O, scene, steps, seed):
@@ -145,8 +185,7 @@ def main():
     restitution = "--restitution" in sys.argv
     from tests.emu import build
     os.environ["B2D_LIB"] = build.build()
-    os.environ["B2D_GRAPH"] = "0"
-    os.environ["B2D_TILES"] = tiles
+    mode = "dataflow" if tiles == "0" else "plain"
     import edyn_b200 as E
     from oracle import oracle as O
     from tests.test_ref_stepper import random_scene, random_scene_wide
@@ -158,7 +197,8 @@ def main():
         return
     for i in range(first, last):
         scene = fixed[i]() if kind == "fixed" else (random_scene_wide if kind == "wide" else random_scene)(E, O, i)
-        res = lockstep_with_mutations(E, O, scene, steps, i) if "--mutate" in sys.argv else lockstep(E, O, scene, steps, restitution)
+        res = lockstep_with_mutations(E, O, scene, steps, i) if "--mutate" in sys.argv else lockstep(E, O, scene, steps, restitution, mode)
+        res.pop("digests", None)
         res["scene"] = scene["name"]
         out.append(res)
     print(json.dumps(dict(results=out, seconds=time.time() - t0)))
