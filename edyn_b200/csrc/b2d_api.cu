@@ -276,11 +276,12 @@ static int check_device_flags(b2d_world *w) {
     w->error = "device error flags:";
     if (err & ERR_MANIFOLD_CAPACITY) w->error += " max_manifolds exceeded;";
     if (err & ERR_LARGE_CAPACITY) w->error += " large-body list overflow;";
-    if (err & ERR_COLOR_OVERFLOW) w->error += " more than 64 constraints of one kind on one dynamic body;";
+    if (err & ERR_COLOR_OVERFLOW) w->error += " a contact or joint found all 64 colours taken on its dynamic bodies together;";
     if (err & ERR_SOLVER_TIMEOUT) w->error += " solver dataflow wait timed out;";
+    if (err & ERR_RESTITUTION_GROUP) w->error += " restitution solver: more than 32 closing manifolds or 96 contact points at one body;";
     if (err & ERR_UNKNOWN_ENTITY) w->error += " hand-over blob names an unknown entity;";
     if (err & (ERR_MANIFOLD_CAPACITY | ERR_LARGE_CAPACITY)) return B2D_ERR_CAPACITY;
-    if (err & ERR_COLOR_OVERFLOW) return B2D_ERR_UNSUPPORTED;
+    if (err & (ERR_COLOR_OVERFLOW | ERR_RESTITUTION_GROUP)) return B2D_ERR_UNSUPPORTED;
     return B2D_ERR_CUDA;
 }
 int b2d_sync(b2d_world *w) { if (!w) return B2D_ERR_ARGUMENT; cudaSetDevice(w->cfg.device); CK(cudaStreamSynchronize(w->stream)); return check_device_flags(w); }
@@ -298,7 +299,9 @@ static float shape_diameter(uint32_t kind, const float *p) {
 // Broadphase classes, world-wide: the grid pitch is the largest bounding diameter among the bodies that go into the
 // grid; planes and bodies much larger than the typical dynamic body (4 x the mean dynamic diameter of the WHOLE world,
 // however the bodies were batched) are kept in a brute-force list instead.  Runs before the first step after the body
-// population changed; results do not depend on the classification (the exact AABB tests decide), only speed does.
+// population changed; results do not depend on the classification (the exact AABB tests decide), only speed does.  A
+// large DYNAMIC body also searches brute force, and its constraints are filed under it, or under its small dynamic
+// partner (key_body): tests/test_gpu_large_bodies.py holds both to the oracle.
 static void class_add(b2d_world *w, float diam, bool dyn) {
     w->diam.push_back(diam); w->isdyn.push_back(dyn ? 1 : 0);
     if (dyn && diam > 0 && std::isfinite(diam)) { w->class_sum += diam; ++w->class_cnt; }
@@ -1345,6 +1348,9 @@ int b2d_upload_bodies(b2d_world *w, uint32_t n, const uint32_t *ids, const b2d_b
     if (p->kind) {
         for (uint32_t k = 0; k < n; ++k) w->isdyn[ids[k]] = p->kind[k] == B2D_DYNAMIC ? 1 : 0;
         w->class_dirty = true;
+        // a constraint coloured while one of its bodies was not dynamic only avoided the other body's colours: a body
+        // that becomes dynamic would bring clashing colours along, so the next step colours everything afresh
+        w->contacts_dirty = true;
     }
     return B2D_OK;
 }

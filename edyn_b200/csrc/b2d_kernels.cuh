@@ -212,9 +212,14 @@ __global__ void k_cell_extent(Dev d, int *out6) {
         if ((threadIdx.x & 31) == 0 && mn[k] <= mx[k]) { atomicMin(&out6[k], mn[k]); atomicMax(&out6[3 + k], mx[k]); }
     }
 }
-B2D_D uint32_t key_body(const Dev &d, uint2 pr) {      // the body a constraint is filed under: its (smaller) dynamic one
-    const uint32_t fa = d.flags[pr.x];
-    return (is_dynamic(fa) && !(fa & F_LARGE)) ? pr.x : pr.y;
+// The body a manifold is filed under (sort key, tile, spatial rank): a dynamic one whenever it has one, the non-large one
+// of two dynamic bodies (its spatial rank is meaningful), a non-dynamic one only when neither is dynamic.  This is the
+// root rule of the island census (k_color_list) and of the hinges' keys (k_color_keys): every constraint of a tiled
+// island sorts into its tile's range, so k_island_tiles / k_solve_tiles see all of a tiled body's constraints and the
+// dataflow path none of them.
+B2D_D uint32_t key_body(const Dev &d, uint2 pr) {
+    const uint32_t fa = d.flags[pr.x], fb = d.flags[pr.y];
+    return (is_dynamic(fa) && (!(fa & F_LARGE) || !is_dynamic(fb))) ? pr.x : pr.y;
 }
 // spatial part of a dataflow manifold's sort key (k_color_keys): the key body's rank in the cell order, 14 bits
 B2D_D uint32_t df_spatial(const Dev &d, uint32_t rank) { return (uint32_t)(((unsigned long long)rank << KEY_DF_SPATIAL_BITS) / d.nbodies); }

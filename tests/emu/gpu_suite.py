@@ -6,8 +6,8 @@ emulation (tests/emu) instead of a GPU: the kernels' logic, the C ABI, the Pytho
 Not run: the full-size configs and the 1000-step box stack (hours under emulation), the hand-over tests (their payloads live
 in torch CUDA tensors), the NCCL tests, the C++ adapter's hello_world (links libb2d.so by name).
 State at the end of round 2: 32 tests, all green (the same tests were green on a GPU before the last kernel clean-up;
-tests/test_zz_gpu_stepper_b2d.py has only ever run here).  The tile-edge and random lock-step files run here with fewer
-steps and seeds and without their CUDA-graph mode (the emulation launches plainly)."""
+tests/test_zz_gpu_stepper_b2d.py has only ever run here).  The tile-edge, random and large-body lock-step files run here with
+fewer steps and seeds and without their CUDA-graph mode (the emulation launches plainly)."""
 import os
 import subprocess
 import sys
@@ -42,7 +42,7 @@ def main():
     import tests.test_zz_gpu_stepper_b2d as Z
     Z.load = load
     files = [os.path.join(ROOT, "tests", f) for f in ("test_gpu_parity.py", "test_gpu_dist.py", "test_gpu_handover.py", "test_zz_gpu_stepper_b2d.py",
-                                                      "test_gpu_tile_edges.py", "test_gpu_random_lockstep.py")]
+                                                      "test_gpu_tile_edges.py", "test_gpu_random_lockstep.py", "test_gpu_large_bodies.py")]
     return pytest.main(["-q", "-m", "gpu", "-k", SELECT, "-p", "no:cacheprovider"] + files + sys.argv[1:])
 
 

@@ -4,7 +4,11 @@ pair lists identical, post-solve state within 1e-5 (here: identical, glibc's sin
 replaying the device's Gauss-Seidel order, manifolds and joint impulses re-synchronised every step.  The -m gpu lock-step
 tests (test_gpu_tile_edges.py, test_gpu_random_lockstep.py) call `lockstep` in-process, on the GPU or the emulation.
 
-    python tests/emu/lockstep.py fixed|narrow|wide FIRST LAST [--tiles 0|1] [--steps N] [--restitution] [--mutate]     -> one JSON line
+    python tests/emu/lockstep.py fixed|narrow|wide|large|beyond FIRST LAST [--tiles 0|1] [--steps N] [--restitution] [--mutate]
+                                 [--bp-warp-max N]     -> one JSON line
+large: scenes with large dynamic bodies (tests/large_scenes.py), within every limit; beyond: the same content past the
+64 colours and the restitution group's 32 manifolds / 96 points, flags only (tiles on: a colour clash on the dataflow
+path would spend the waits' whole spin budget).
 Runs in its own process because B2D_LIB has to be set before edyn_b200 is imported."""
 import json
 import os
@@ -24,12 +28,14 @@ MODES = {"plain": dict(B2D_GRAPH="0", B2D_GRAPH_REUSE="1", B2D_TILES="1"),
 STATE_KEYS = ("pos", "orn", "linvel", "angvel", "aabb")
 
 
-def build_world(E, scene, mode=None, **kw):
-    """E.scenes.build_world with the environment of `mode` (read when the world is created); None: as the environment is."""
-    if mode is None:
+def build_world(E, scene, mode=None, env=None, **kw):
+    """E.scenes.build_world with the environment of `mode` (read when the world is created) and the extra variables `env`;
+    None: as the environment is."""
+    env = {**(MODES[mode] if mode is not None else {}), **(env or {})}
+    if not env:
         return E.scenes.build_world(scene, **kw)
-    saved = {k: os.environ.get(k) for k in MODES[mode]}
-    os.environ.update(MODES[mode])
+    saved = {k: os.environ.get(k) for k in env}
+    os.environ.update(env)
     try:
         return E.scenes.build_world(scene, **kw)
     finally:
@@ -40,11 +46,15 @@ def build_world(E, scene, mode=None, **kw):
                 os.environ[k] = v
 
 
-def lockstep(E, O, scene, steps, restitution_solver=False, mode=None, hook=None, vel_iters=None, pos_iters=None):
+def lockstep(E, O, scene, steps, restitution_solver=False, mode=None, hook=None, vel_iters=None, pos_iters=None, env=None,
+             before=None, max_bodies=None):
     """One device world in `mode` (a key of MODES; None: as the environment says) against the oracle, `steps` single
-    steps.  vel_iters / pos_iters override the scene's settings on both sides; hook(step, world) runs after each step's comparison (and may assert).  Returns ok, worst
-    (largest state difference), exact (bit-identical steps), points (contact points at the end), max_points (most points
-    in one manifold at any step), flags, and digests: one hash of the device state per step, for comparing modes."""
+    steps.  vel_iters / pos_iters override the scene's settings on both sides; env: more environment variables for the
+    world's creation; hook(step, world) runs after each step's comparison (and may assert); before(step, world, oracle)
+    runs before each step, may change both worlds and returns the oracle to continue with; max_bodies reserves room for
+    bodies added on the way.  Returns ok, worst (largest state difference), exact (bit-identical steps), points (contact
+    points at the end), max_points (most points in one manifold at any step), flags, and digests: one hash of the device
+    state and ordered pair set per step, for comparing modes."""
     import hashlib
     import numpy as np
     st = dict(scene["settings"])
@@ -52,7 +62,7 @@ def lockstep(E, O, scene, steps, restitution_solver=False, mode=None, hook=None,
         st["velocity_iterations"] = vel_iters
     if pos_iters is not None:
         st["position_iterations"] = pos_iters
-    w = build_world(E, scene, mode, flags=E.world.FLAG_RESTITUTION_SOLVER if restitution_solver else 0, **st)
+    w = build_world(E, scene, mode, env, flags=E.world.FLAG_RESTITUTION_SOLVER if restitution_solver else 0, max_bodies=max_bodies, **st)
     o = O.OracleWorld(vel_iters=st["velocity_iterations"], pos_iters=st["position_iterations"])
     if restitution_solver:
         o.set_restitution_iterations(8, 3)          # no graph order handed over: the oracle's defaults are the device's conventions
@@ -64,13 +74,16 @@ def lockstep(E, O, scene, steps, restitution_solver=False, mode=None, hook=None,
         o.add_exclusions(*scene["exclusions"])
     worst, exact, max_points, digests = 0.0, 0, 0, []
     for s in range(steps):
+        if before is not None:
+            o = before(s, w, o)
         w.step(1)
         hi, pr = w.solver_order()
         o.run_phases(O.PH_BROAD | O.PH_NARROW | O.PH_ISLANDS)
         o.set_order(hi, pr)
         o.run_phases(O.PH_SOLVE)
         g, c = w.download_state(), o.state()
-        if {tuple(p) for p in w.pairs().tolist()} != {tuple(p) for p in o.pairs().tolist()}:
+        wp = w.pairs()
+        if {tuple(p) for p in wp.tolist()} != {tuple(p) for p in o.pairs().tolist()}:
             return dict(ok=False, step=s, why="ordered broadphase pair lists differ")
         if not np.array_equal(w.islands(), o.islands()):
             return dict(ok=False, step=s, why="island labels differ")
@@ -79,7 +92,8 @@ def lockstep(E, O, scene, steps, restitution_solver=False, mode=None, hook=None,
         exact += err == 0.0
         if err > 1e-5:
             return dict(ok=False, step=s, why=f"state differs by {err:.3e}")
-        digests.append(hashlib.sha1(b"".join(np.ascontiguousarray(g[k]).tobytes() for k in STATE_KEYS)).hexdigest())
+        wp = wp[np.lexsort((wp[:, 1], wp[:, 0]))] if len(wp) else wp
+        digests.append(hashlib.sha1(b"".join(np.ascontiguousarray(x).tobytes() for x in [g[k] for k in STATE_KEYS] + [wp])).hexdigest())
         o.set_state(g["pos"], g["orn"], g["linvel"], g["angvel"])
         gc = w.contacts()
         max_points = max(max_points, int(gc["num"].max(initial=0)))
@@ -91,7 +105,22 @@ def lockstep(E, O, scene, steps, restitution_solver=False, mode=None, hook=None,
     stats = w.stats()
     w.close()
     return dict(ok=stats["error_flags"] == 0, worst=worst, exact=exact, points=int(stats["contact_points"]), max_points=max_points,
-                flags=int(stats["error_flags"]), reused=int(stats["steps_reused"]), digests=digests)
+                flags=int(stats["error_flags"]), reused=int(stats["steps_reused"]), colors=int(stats["contact_colors"]), digests=digests)
+
+
+def over_the_limit(E, scene, steps, restitution_solver=False):
+    """The device alone, `steps` steps of a scene beyond one of its limits: the error flags and what World.sync() raises
+    (None: nothing).  No oracle: past a limit the state is not meant to match."""
+    w = build_world(E, scene, None, flags=E.world.FLAG_RESTITUTION_SOLVER if restitution_solver else 0, **scene["settings"])
+    w.step(steps)
+    flags = int(w.stats()["error_flags"])
+    try:
+        w.sync()
+        raised = None
+    except E.world.B2DError as e:
+        raised = str(e)
+    w.close()
+    return dict(ok=True, flags=flags, raised=raised)
 
 
 def lockstep_with_mutations(E, O, scene, steps, seed):
@@ -189,6 +218,10 @@ def main():
     import edyn_b200 as E
     from oracle import oracle as O
     from tests.test_ref_stepper import random_scene, random_scene_wide
+    from tests import large_scenes as L
+    env = {"B2D_BP_WARP_MAX": sys.argv[sys.argv.index("--bp-warp-max") + 1]} if "--bp-warp-max" in sys.argv else None
+    large = [lambda name=name: L.SCENES[name](E) for name in L.SCENES] + [lambda k=k: L.plank_degree(E, k) for k in (32, 33, 63, 64)]
+    beyond = [(lambda: L.plank_degree(E, 65), False), (lambda: L.plank_bounce(E, 33), True), (lambda: L.plank_bounce(E, 25, boxes=True), True)]
     fixed = [lambda: E.scenes.hello_world(), lambda: E.scenes.boxes_on_plane(3), lambda: E.scenes.spheres_in_box(4, 6, 4),
              lambda: E.scenes.mixed_pile(5, jitter=0.01), lambda: E.scenes.hinge_chains(2, 2)]
     out, t0 = [], time.time()
@@ -196,8 +229,17 @@ def main():
         print(json.dumps(dict(results=free_run_against_real_stepper(E, O), seconds=0.0)))
         return
     for i in range(first, last):
-        scene = fixed[i]() if kind == "fixed" else (random_scene_wide if kind == "wide" else random_scene)(E, O, i)
-        res = lockstep_with_mutations(E, O, scene, steps, i) if "--mutate" in sys.argv else lockstep(E, O, scene, steps, restitution, mode)
+        if kind == "beyond":
+            make, rest = beyond[i]
+            scene = make()
+            res = over_the_limit(E, scene, steps, rest)
+        elif kind == "large":
+            scene = large[i]()
+            res = lockstep(E, O, scene, steps, restitution, mode, env=env)
+            res["large"], res["want"] = L.large_dynamic(scene["bodies"]).tolist(), scene["large"]
+        else:
+            scene = fixed[i]() if kind == "fixed" else (random_scene_wide if kind == "wide" else random_scene)(E, O, i)
+            res = lockstep_with_mutations(E, O, scene, steps, i) if "--mutate" in sys.argv else lockstep(E, O, scene, steps, restitution, mode)
         res.pop("digests", None)
         res["scene"] = scene["name"]
         out.append(res)

@@ -17,8 +17,9 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def _run(kind, first, last, tiles="1", steps=80, restitution=False, mutate=False):
+def _run(kind, first, last, tiles="1", steps=80, restitution=False, mutate=False, extra=()):
     cmd = [sys.executable, os.path.join(ROOT, "tests", "emu", "lockstep.py"), kind, str(first), str(last), "--tiles", tiles, "--steps", str(steps)]
+    cmd += list(extra)
     if restitution:
         cmd.append("--restitution")
     if mutate:
@@ -79,3 +80,32 @@ def test_emulated_kernels_against_the_real_stepper_directly(O):
             assert res["dpos"] == 0.0 and res["dvel"] == 0.0, res
         else:
             assert res["dpos"] <= 1e-6 and res["dvel"] <= 1e-6, res
+
+
+@pytest.mark.parametrize("tiles,search", [("1", "warp"), ("0", "warp"), ("1", "thread")])
+def test_emulated_large_dynamic_bodies(O, tiles, search):
+    """tests/large_scenes.py within every limit (a few steps each; tests/test_gpu_large_bodies.py runs them long): a plank
+    alone on the plane, tipping from an edge onto its face, a log and a plank with bodies dropped on them, crates against
+    static, kinematic and each other, and a plank at 32, 33, 63 and 64 manifolds -- with the island tiles, on the dataflow
+    path, and with the thread-per-body neighbourhood search (B2D_BP_WARP_MAX=0)."""
+    extra = ("--bp-warp-max", "0") if search == "thread" else ()
+    res = _run("large", 0, 11, tiles=tiles, steps=12, extra=extra)
+    assert len(res) == 11
+    for r in res:
+        assert r["ok"] and r["worst"] == 0.0 and r["exact"] == 12, r
+        assert r["large"] and r["large"] == r["want"], r
+        if r["scene"].startswith("plank_degree_"):
+            assert r["colors"] == int(r["scene"].rsplit("_", 1)[1]), r
+
+
+def test_emulated_limits_are_flagged():
+    """One body past the limits: 65 manifolds on a plank overflow the 64 colours (ERR_COLOR_OVERFLOW), 33 closing
+    manifolds and 100 closing contact points at the plank overflow a restitution group (ERR_RESTITUTION_GROUP); World.sync()
+    raises with the library's message.  The flags only: past a limit the state is not meant to match, and these cases stay
+    off the GPU (on the dataflow path a colour clash can spend the waits' whole spin budget)."""
+    res = {r["scene"]: r for r in _run("beyond", 0, 3, steps=2)}
+    assert res["plank_degree_65"]["flags"] == 2, res
+    assert "all 64 colours taken" in res["plank_degree_65"]["raised"], res
+    for name in ("plank_bounce_33", "plank_bounce_25_boxes"):
+        assert res[name]["flags"] == 32, res
+        assert "restitution solver: more than 32 closing manifolds or 96 contact points" in res[name]["raised"], res
