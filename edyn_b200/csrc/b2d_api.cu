@@ -28,7 +28,7 @@ struct b2d_world {
     std::string error;
     int num_sms = 0;
     int coop_blocks_color = 0, coop_blocks_df = 0, coop_blocks_pos_df = 0;
-    int tile_blocks = 0, tile_fused_blocks = 0, tile_fused_blocks_2p = 0;     // grids of the island-tile kernels (CTAs loop over the tiles)
+    int tile_fused_blocks = 0, tile_fused_blocks_2p = 0;     // grids of the island-tile kernels (CTAs loop over the tiles)
     int cell_key_bits = 48;                         // sum of d.cell_bits: end bit of the cell sort
     uint32_t bp_warp_max = 100000;                  // neighbourhood search: warp per body up to this many bodies (B2D_BP_WARP_MAX)
     void *cub_tmp = nullptr; size_t cub_tmp_bytes = 0;
@@ -231,8 +231,6 @@ b2d_world *b2d_create(const b2d_config *cfg) {
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_color, 256, 0); w->coop_blocks_color = std::max(1, std::min(per_sm, want)) * w->num_sms;
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_solve_df, B2D_SOLVE_THREADS, 0); w->coop_blocks_df = std::max(1, per_sm) * w->num_sms;
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_position_df, B2D_POS_THREADS, 0); w->coop_blocks_pos_df = std::max(1, per_sm) * w->num_sms;
-    cudaFuncSetAttribute(k_solve_tiles, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TILE_SOLVE_SMEM);
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_solve_tiles, TILE_CAP, TILE_SOLVE_SMEM); w->tile_blocks = std::max(1, per_sm) * w->num_sms;
     cudaFuncSetAttribute(k_island_tiles, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TILE_FUSED_SMEM);
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_island_tiles, TILE_CAP, TILE_FUSED_SMEM); w->tile_fused_blocks = std::max(1, per_sm) * w->num_sms;
     cudaFuncSetAttribute(k_island_tiles_2p, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TILE_FUSED_SMEM_2P);
@@ -669,9 +667,8 @@ static int enqueue_rebuild(b2d_world *w, int recolor) {
 }
 static int enqueue_prepare(b2d_world *w) {
     Dev &d = w->d;
-    const int fused = (d.max_tiles && w->cfg.position_iterations > 0) ? 1 : 0;        // k_island_tiles prepares the tiled rows
-    LAUNCH(k_prepare_contacts, d.NM, 256, d, fused);
-    if (d.nhinges) LAUNCH(k_prepare_hinges, d.nhinges, 256, d, fused);
+    LAUNCH(k_prepare_contacts, d.NM, 256, d);
+    if (d.nhinges) LAUNCH(k_prepare_hinges, d.nhinges, 256, d);
     return B2D_OK;
 }
 static int enqueue_solver_a(b2d_world *w, int recolor) {
@@ -685,28 +682,22 @@ static int enqueue_solver_b(b2d_world *w) {
     // The two schedules work on disjoint islands.  (Forking the tile kernel onto a second stream was measured: no gain --
     // the cooperative launch wants the whole machine and waits for the tiles, or the tiles wait for it.)
     const int pi = (int)w->cfg.position_iterations;
-    if (d.max_tiles) {
-        // with position iterations: the tiled islands' whole solver.update in one launch; without: the velocity part alone
-        if (pi > 0) {       // two-point tiles [0, ntiles2), then the generic ones
-            k_island_tiles_2p<<<w->tile_fused_blocks_2p, TILE_CAP, TILE_FUSED_SMEM_2P, w->stream>>>(d, vi, pi); ++w->launches;
-            k_island_tiles<<<w->tile_fused_blocks, TILE_CAP, TILE_FUSED_SMEM, w->stream>>>(d, vi, pi); ++w->launches;
-        }
-        else { k_solve_tiles<<<w->tile_blocks, TILE_CAP, TILE_SOLVE_SMEM, w->stream>>>(d, vi); ++w->launches; }
+    if (d.max_tiles) {      // the tiled islands' whole solver.update: two-point tiles [0, ntiles2), then the generic ones
+        k_island_tiles_2p<<<w->tile_fused_blocks_2p, TILE_CAP, TILE_FUSED_SMEM_2P, w->stream>>>(d, vi, pi); ++w->launches;
+        k_island_tiles<<<w->tile_fused_blocks, TILE_CAP, TILE_FUSED_SMEM, w->stream>>>(d, vi, pi); ++w->launches;
     }
     CK(coop_launch(w, k_solve_df, w->coop_blocks_df, B2D_SOLVE_THREADS, d, vi));
     return B2D_OK;
 }
 static int enqueue_integrate(b2d_world *w) {
     Dev &d = w->d;
-    const int fused = (d.max_tiles && w->cfg.position_iterations > 0) ? 1 : 0;      // k_island_tiles has integrated the tiled bodies
-    LAUNCH(k_integrate, d.nbodies, 256, d, w->cfg.position_iterations == 0 ? 1 : 0, fused);
+    LAUNCH(k_integrate, d.nbodies, 256, d, w->cfg.position_iterations == 0 ? 1 : 0);
     return B2D_OK;
 }
 static int enqueue_solver_c(b2d_world *w) {
     Dev &d = w->d;
     const int pi = (int)w->cfg.position_iterations;
-    const int fused = (d.max_tiles && pi > 0) ? 1 : 0;
-    LAUNCH(k_store_impulses, d.NM, 256, d, fused);
+    LAUNCH(k_store_impulses, d.NM, 256, d);
     if (pi > 0) {
         CK(coop_launch(w, k_position_df, w->coop_blocks_pos_df, B2D_POS_THREADS, d, pi));
         LAUNCH(k_finalize, d.nbodies, 256, d);

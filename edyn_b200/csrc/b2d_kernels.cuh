@@ -215,8 +215,8 @@ __global__ void k_cell_extent(Dev d, int *out6) {
 // The body a manifold is filed under (sort key, tile, spatial rank): a dynamic one whenever it has one, the non-large one
 // of two dynamic bodies (its spatial rank is meaningful), a non-dynamic one only when neither is dynamic.  This is the
 // root rule of the island census (k_color_list) and of the hinges' keys (k_color_keys): every constraint of a tiled
-// island sorts into its tile's range, so k_island_tiles / k_solve_tiles see all of a tiled body's constraints and the
-// dataflow path none of them.
+// island sorts into its tile's range, so k_island_tiles sees all of a tiled body's constraints and the dataflow path none
+// of them.
 B2D_D uint32_t key_body(const Dev &d, uint2 pr) {
     const uint32_t fa = d.flags[pr.x], fb = d.flags[pr.y];
     return (is_dynamic(fa) && (!(fa & F_LARGE) || !is_dynamic(fb))) ? pr.x : pr.y;
@@ -916,7 +916,7 @@ __global__ void __launch_bounds__(256) k_color(Dev d) {
 }
 
 // ---- island tiles.  An island with at most TILE_ISLAND_MAX dynamic bodies, manifolds with points and joints is solved
-// inside one CTA (k_island_tiles; k_solve_tiles when there are no position iterations).  Islands are packed into tiles in root-id order: with weight
+// inside one CTA (k_island_tiles).  Islands are packed into tiles in root-id order: with weight
 // w = max(bodies, manifolds, joints) <= TILE_ISLAND_MAX per island and P the exclusive prefix sum of the weights, island
 // -> tile P / g with g = TILE_CAP + 1 - (heaviest tiled island) puts at most TILE_CAP of each into every tile.  Which islands
 // are tiled changes speed, never results: the per-body constraint order is fixed by the colours alone.
@@ -1129,10 +1129,10 @@ B2D_D void hinge_rows(const Dev &d, uint32_t h, const SBody &A, const SBody &B, 
     R[6 * stride] = make_float4(imp[2], imp[3], imp[4], 0);
 }
 
-// Row preparation per sorted manifold; rows are written in colour order so the solve kernel streams them.  With fused
-// != 0 k_island_tiles prepares the tiled range [0, ntiled) itself and this kernel starts after it.
-__global__ void __launch_bounds__(256) k_prepare_contacts(Dev d, int fused) {
-    const uint32_t n = d.cnt->nactive, first = fused ? d.cnt->ntiled : 0u;
+// Row preparation per sorted manifold; rows are written in colour order so the solve kernel streams them.
+// k_island_tiles prepares the tiled range [0, ntiled) itself and this kernel starts after it.
+__global__ void __launch_bounds__(256) k_prepare_contacts(Dev d) {
+    const uint32_t n = d.cnt->nactive, first = d.cnt->ntiled;
     GRID_STRIDE(j, n - first) {
         const uint32_t i = first + j;
         uint32_t m = d.cidx_s[i];
@@ -1168,9 +1168,9 @@ __global__ void __launch_bounds__(256) k_prepare_contacts(Dev d, int fused) {
     }
 }
 
-// per sorted hinge; fused as in k_prepare_contacts ([0, nhtiled) is prepared by k_island_tiles)
-__global__ void k_prepare_hinges(Dev d, int fused) {
-    const uint32_t n = d.cnt->nhactive, first = fused ? d.cnt->nhtiled : 0u;
+// per sorted hinge; [0, nhtiled) is prepared by k_island_tiles
+__global__ void k_prepare_hinges(Dev d) {
+    const uint32_t n = d.cnt->nhactive, first = d.cnt->nhtiled;
     GRID_STRIDE(j, n - first) {
         const uint32_t i = first + j;
         uint32_t h = d.hidx_s[i];
@@ -1202,7 +1202,7 @@ __global__ void k_prepare_hinges(Dev d, int fused) {
 // The reference sweeps the rows of an island serially (island_solver.cpp:94-111): per iteration all joint rows, all
 // contact normal rows, then all friction pairs.  Here the constraints of a type are coloured so that a colour touches
 // disjoint dynamic bodies; any schedule that runs a body's constraints in (iteration, type, colour) order produces the
-// bits of a serial sweep in that order.  Two schedules do: k_solve_tiles for small islands (everything on chip,
+// bits of a serial sweep in that order.  Two schedules do: k_island_tiles for small islands (everything on chip,
 // __syncthreads between colours) and k_solve_df for the rest (per-body tickets in global memory).
 
 struct VBody { v3 dv, dw; float inv_m; m3 inv_I; uint32_t id; bool proc; float pad1, pad2; };
@@ -1263,8 +1263,13 @@ B2D_D void frow_solve(const float4 &r0, const float4 &r1, const float4 &r2, cons
     apply_imp_f(A, B, t, T1, T2, T3, d0);
     apply_imp_f(A, B, u, U1, U2, U3, d1);
 }
-// the five rows of a plain hinge (hinge_constraint.cpp:26-69): three point rows, two angular rows
-B2D_D void hinge_solve(v3 rA, v3 rB, v3 p, v3 q, const float em[5], const float rhs[5], float imp[5], VBody &A, VBody &B, bool warm) {
+// the five rows of a plain hinge (hinge_constraint.cpp:26-69): three point rows, two angular rows; r0..r6 as hinge_rows
+// writes them, the impulses repacked into r5 / r6 (unchanged by the warm start)
+B2D_D void hinge_solve(const float4 &r0, const float4 &r1, const float4 &r2, const float4 &r3, const float4 &r4, float4 &r5, float4 &r6,
+                       VBody &A, VBody &B, bool warm) {
+    const v3 rA = mk3(r0), rB = mk3(r1), p = mk3(r2), q = mk3(r3);
+    const float em[5] = {r0.w, r1.w, r2.w, r3.w, r4.x}, rhs[5] = {r4.y, r4.z, r4.w, r5.x, r5.y};
+    float imp[5] = {r5.z, r5.w, r6.x, r6.y, r6.z};
     #pragma unroll
     for (int k = 0; k < 5; ++k) {
         v3 J0, J1, J2, J3;
@@ -1279,130 +1284,7 @@ B2D_D void hinge_solve(v3 rA, v3 rB, v3 p, v3 q, const float em[5], const float 
         else delta = solve_row(rhs[k], em[k], -SCALAR_MAX, SCALAR_MAX, imp[k], rel_speed(J0, J1, J2, J3, A.dv, A.dw, B.dv, B.dw));
         apply_imp(A, B, J0, J1, J2, J3, delta);
     }
-}
-
-// ---------------------------------------------------------------------- island tiles: everything on chip
-// One CTA per tile, thread t owns joint t and contact manifold t of the tile for ALL iterations: the rows of the first
-// two contact points stay in registers, those of points 3 and 4 (box faces), the joint rows and the body records (delta
-// velocities + world inverse inertia) in shared memory.  Rows are read from DRAM once per step
-// instead of once per iteration, and colours are separated by __syncthreads instead of tickets.
-// shared memory of a tile: body records (dv, dw, inverse inertia rows | inverse mass), joint rows, rows of contact points 3 and 4
-constexpr size_t TILE_SOLVE_SMEM = (5 + 7 + 10) * TILE_CAP * sizeof(float4);
-B2D_D void tb_load(const float4 *sb, uint32_t tag, uint32_t slot, VBody &b) {
-    b.proc = !(tag & 0x80000000u); b.id = tag & 0x7FFFFFFFu;
-    if (b.proc) {
-        const float4 *r = sb + 5 * slot;
-        const float4 a = r[0], w = r[1], r0 = r[2], r1 = r[3], r2 = r[4];
-        b.dv = mk3(a); b.dw = mk3(w); b.inv_m = r0.w; b.inv_I.r0 = mk3(r0); b.inv_I.r1 = mk3(r1); b.inv_I.r2 = mk3(r2);
-    } else { b.dv = mk3(0, 0, 0); b.dw = mk3(0, 0, 0); b.inv_m = 0; b.inv_I = m3_zero(); }
-}
-B2D_D void tb_store(float4 *sb, uint32_t slot, const VBody &b) {
-    if (b.proc) { sb[5 * slot] = f4(b.dv, 0); sb[5 * slot + 1] = f4(b.dw, 0); }
-}
-__global__ void __launch_bounds__(TILE_CAP, 2) k_solve_tiles(Dev d, int iters) {
-    extern __shared__ float4 s_tile[];                     // TILE_SOLVE_SMEM bytes
-    float4 *s_body = s_tile;                               // 5 float4 per body
-    float4 *s_hr = s_tile + 5 * TILE_CAP;                  // joint rows, row-major over the tile's joints (conflict-free)
-    float4 *s_row = s_tile + 12 * TILE_CAP;                // contact points 3 and 4: (R0 R1 R2 R3 IMP) x 2, same layout
-    __shared__ uint32_t s_ncol[2];
-    const uint32_t ntiles = d.cnt->ntiles, t = threadIdx.x;
-    const size_t NM = d.NM;
-    for (uint32_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-        const uint32_t nb = min(d.tile_nb[tile], (uint32_t)TILE_CAP);
-        const uint32_t c0 = d.tile_c0[tile], c1 = min(d.tile_c1[tile], c0 + TILE_CAP), h0 = d.tile_h0[tile], h1 = min(d.tile_h1[tile], h0 + TILE_CAP);
-        if (t < 2) s_ncol[t] = 0;
-        if (t < nb) {
-            const uint32_t b = d.tile_body[(size_t)tile * TILE_CAP + t];
-            float4 *r = s_body + 5 * t;
-            r[0] = make_float4(0, 0, 0, 0); r[1] = make_float4(0, 0, 0, 0);
-            r[2] = d.invIW[3 * b]; r[3] = d.invIW[3 * b + 1]; r[4] = d.invIW[3 * b + 2];
-        }
-        __syncthreads();
-        const bool hasH = h0 + t < h1, hasC = c0 + t < c1;
-        const uint32_t hi = h0 + t, ci = c0 + t;
-        uint4 hh = make_uint4(0, 0, 0, 0), ch = make_uint4(0, 0, 0, 0);
-        uint32_t hcol = 0xFFu, ccol = 0xFFu;
-        float4 a0, a1, a2, a3, aim, b0, b1, b2, b3, bim;      // rows of contact points 1 and 2
-        a0 = a1 = a2 = a3 = aim = b0 = b1 = b2 = b3 = bim = make_float4(0, 0, 0, 0);
-        if (hasH) {
-            hh = d.hhdr[hi]; hcol = d.hkey_s[hi] & 63u;
-            const float4 *R = d.HR + 7 * (size_t)hi;
-            #pragma unroll
-            for (int k = 0; k < 7; ++k) s_hr[k * TILE_CAP + t] = R[k];
-            atomicMax(&s_ncol[0], hcol + 1u);
-        }
-        if (hasC) {
-            ch = d.hdr[ci]; ccol = d.ckey_s[ci] & 63u;
-            a0 = d.R0[ci]; a1 = d.R1[ci]; a2 = d.R2[ci]; a3 = d.R3[ci]; aim = d.IMP[ci];
-            if (ch.z > 1) { b0 = d.R0[NM + ci]; b1 = d.R1[NM + ci]; b2 = d.R2[NM + ci]; b3 = d.R3[NM + ci]; bim = d.IMP[NM + ci]; }
-            for (uint32_t s = 2; s < ch.z; ++s) {
-                const size_t ri = s * NM + ci;
-                float4 *r = s_row + (s - 2) * 5 * TILE_CAP + t;
-                r[0] = d.R0[ri]; r[TILE_CAP] = d.R1[ri]; r[2 * TILE_CAP] = d.R2[ri]; r[3 * TILE_CAP] = d.R3[ri]; r[4 * TILE_CAP] = d.IMP[ri];
-            }
-            atomicMax(&s_ncol[1], ccol + 1u);
-        }
-        __syncthreads();
-        const uint32_t nhc = s_ncol[0], ncc = s_ncol[1];
-        for (int it = -1; it < iters; ++it) {
-            const bool warm = it < 0;
-            for (uint32_t c = 0; c < nhc; ++c) {
-                if (hcol == c) {
-                    const float4 r0 = s_hr[t], r1 = s_hr[TILE_CAP + t], r2 = s_hr[2 * TILE_CAP + t], r3 = s_hr[3 * TILE_CAP + t],
-                                 r4 = s_hr[4 * TILE_CAP + t], r5 = s_hr[5 * TILE_CAP + t], r6 = s_hr[6 * TILE_CAP + t];
-                    const float em[5] = {r0.w, r1.w, r2.w, r3.w, r4.x}, rhs[5] = {r4.y, r4.z, r4.w, r5.x, r5.y};
-                    float imp[5] = {r5.z, r5.w, r6.x, r6.y, r6.z};
-                    VBody A, B; tb_load(s_body, hh.x, hh.w & 0xFFFFu, A); tb_load(s_body, hh.y, hh.w >> 16, B);
-                    hinge_solve(mk3(r0), mk3(r1), mk3(r2), mk3(r3), em, rhs, imp, A, B, warm);
-                    tb_store(s_body, hh.w & 0xFFFFu, A); tb_store(s_body, hh.w >> 16, B);
-                    if (!warm) { s_hr[5 * TILE_CAP + t] = make_float4(r5.x, r5.y, imp[0], imp[1]); s_hr[6 * TILE_CAP + t] = make_float4(imp[2], imp[3], imp[4], 0); }
-                }
-                __syncthreads();
-            }
-            for (uint32_t c = 0; c < ncc; ++c) {
-                if (ccol == c) {
-                    VBody A, B; tb_load(s_body, ch.x, ch.w & 0xFFFFu, A); tb_load(s_body, ch.y, ch.w >> 16, B);
-                    nrow_solve(a0, a1, a2, aim, A, B, warm);
-                    if (ch.z > 1) nrow_solve(b0, b1, b2, bim, A, B, warm);
-                    for (uint32_t s = 2; s < ch.z; ++s) {
-                        float4 *r = s_row + (s - 2) * 5 * TILE_CAP + t;
-                        float4 im = r[4 * TILE_CAP];
-                        nrow_solve(r[0], r[TILE_CAP], r[2 * TILE_CAP], im, A, B, warm);
-                        r[4 * TILE_CAP] = im;
-                    }
-                    tb_store(s_body, ch.w & 0xFFFFu, A); tb_store(s_body, ch.w >> 16, B);
-                }
-                __syncthreads();
-            }
-            for (uint32_t c = 0; c < ncc; ++c) {
-                if (ccol == c) {
-                    VBody A, B; tb_load(s_body, ch.x, ch.w & 0xFFFFu, A); tb_load(s_body, ch.y, ch.w >> 16, B);
-                    frow_solve(a0, a1, a2, a3, aim, A, B, warm);
-                    if (ch.z > 1) frow_solve(b0, b1, b2, b3, bim, A, B, warm);
-                    for (uint32_t s = 2; s < ch.z; ++s) {
-                        float4 *r = s_row + (s - 2) * 5 * TILE_CAP + t;
-                        float4 im = r[4 * TILE_CAP];
-                        frow_solve(r[0], r[TILE_CAP], r[2 * TILE_CAP], r[3 * TILE_CAP], im, A, B, warm);
-                        r[4 * TILE_CAP] = im;
-                    }
-                    tb_store(s_body, ch.w & 0xFFFFu, A); tb_store(s_body, ch.w >> 16, B);
-                }
-                __syncthreads();
-            }
-        }
-        // results: impulses for the warm-start cache, delta velocities for k_integrate
-        if (hasH) { float4 *R = d.HR + 7 * (size_t)hi; R[5] = s_hr[5 * TILE_CAP + t]; R[6] = s_hr[6 * TILE_CAP + t]; }
-        if (hasC) {
-            d.IMP[ci] = aim; if (ch.z > 1) d.IMP[NM + ci] = bim;
-            for (uint32_t s = 2; s < ch.z; ++s) d.IMP[s * NM + ci] = s_row[((s - 2) * 5 + 4) * TILE_CAP + t];
-        }
-        if (t < nb) {
-            const uint32_t b = d.tile_body[(size_t)tile * TILE_CAP + t];
-            const float4 a = s_body[5 * t], w = s_body[5 * t + 1];
-            d.dvw[2 * b] = make_float4(a.x, a.y, a.z, 0.0f); d.dvw[2 * b + 1] = make_float4(w.x, w.y, w.z, 0.0f);
-        }
-        __syncthreads();
-    }
+    r5 = make_float4(r5.x, r5.y, imp[0], imp[1]); r6 = make_float4(imp[2], imp[3], imp[4], 0);
 }
 
 // ---------------------------------------------------------------------- dataflow: per-body tickets in global memory
@@ -1482,14 +1364,12 @@ B2D_D void hinge_pass(const Dev &d, uint32_t i, bool warm, int pass, uint32_t ma
     const Ticket tk = ticket_of(d.htkt[i], pass, 0, mask);
     VBody A, B; vb_static(d, hd.x, A); vb_static(d, hd.y, B);
     bool pending = true; uint32_t spins = 0;
-    const float em[5] = {r0.w, r1.w, r2.w, r3.w, r4.x}, rhs[5] = {r4.y, r4.z, r4.w, r5.x, r5.y};
-    float imp[5] = {r5.z, r5.w, r6.x, r6.y, r6.z};
     do {
     const bool ok = pending && acquire_try(d, tk, A, B);
     if (ok) {
-    hinge_solve(mk3(r0), mk3(r1), mk3(r2), mk3(r3), em, rhs, imp, A, B, warm);
+    hinge_solve(r0, r1, r2, r3, r4, r5, r6, A, B, warm);
     bodies_publish(d, tk, A, B);
-    if (!warm) { R[5] = make_float4(r5.x, r5.y, imp[0], imp[1]); R[6] = make_float4(imp[2], imp[3], imp[4], 0); }
+    if (!warm) { R[5] = r5; R[6] = r6; }
     pending = false;
     }
     if (!acquire_more(d, tk, pending, ok, spins)) break;
@@ -1633,9 +1513,9 @@ __global__ void __launch_bounds__(B2D_SOLVE_THREADS, 2) k_solve_df(Dev d, int it
 }
 
 // assign_applied_impulses (island_solver.cpp:232-248): rows -> warm-start cache of the constraints.
-__global__ void k_store_impulses(Dev d, int fused) {
+__global__ void k_store_impulses(Dev d) {
     const uint32_t n = d.cnt->nactive, nh = d.cnt->nhactive;
-    const uint32_t first = fused ? d.cnt->ntiled : 0u, hfirst = fused ? d.cnt->nhtiled : 0u;       // k_island_tiles stored its own
+    const uint32_t first = d.cnt->ntiled, hfirst = d.cnt->nhtiled;       // k_island_tiles stored its own
     GRID_STRIDE(k, n - first) {
         const uint32_t i = first + k;
         const uint32_t npts = d.hdr[i].z, m = d.cidx_s[i];
@@ -1653,22 +1533,33 @@ __global__ void k_store_impulses(Dev d, int fused) {
 
 // ====================================================================== integration and refresh
 
-// integrate_velocities (island_solver.cpp:358-376); with refresh != 0 also update_aabbs + update_inertias
-// (solver.cpp:453-465) fused in, used when no position iterations run in between.
-__global__ void __launch_bounds__(256) k_integrate(Dev d, int refresh, int fused) {
+// integrate_velocities (island_solver.cpp:358-376) of one body: the delta velocities of the solve, then position and
+// orientation.  Shared by k_integrate and k_island_tiles.
+B2D_D void integrate_body(v3 &v, v3 &w, v3 &pos, q4 &orn, v3 dv, v3 dw, float dt) {
+    v += dv; w += dw;
+    pos += v * dt;
+    orn = integrate(orn, w, dt);
+}
+// integrate_velocities of the bodies outside the island tiles (k_island_tiles integrates its own); with refresh != 0
+// also update_aabbs + update_inertias (solver.cpp:453-465) of every dynamic body, tiled ones included, for when no
+// position iterations run in between.
+__global__ void __launch_bounds__(256) k_integrate(Dev d, int refresh) {
     if (blockIdx.x == 0 && threadIdx.x == 0) d.cnt->bar = 0;       // grid barrier counter of k_position_df
     GRID_STRIDE(i, d.nbodies) {
         uint32_t f = d.flags[i];
         if (!is_dynamic(f)) continue;
-        if (fused && d.btile[i] != TILE_NONE) continue;             // integrated by k_island_tiles
+        const bool tiled = d.btile[i] != TILE_NONE;
+        if (tiled && !refresh) continue;
         float4 p4 = d.pos[i];
-        v3 v = mk3(d.linvel[i]), w = mk3(d.angvel[i]);
-        v += mk3(d.dvw[2 * i]); w += mk3(d.dvw[2 * i + 1]);
-        v3 pos = mk3(p4); pos += v * d.dt;
-        q4 orn = integrate(mkq(d.orn[i]), w, d.dt);
-        d.linvel[i] = f4(v, 0); d.angvel[i] = f4(w, 0);
-        d.pos[i] = f4(pos, p4.w); d.orn[i] = f4(orn);
-        d.dvw[2 * i] = make_float4(0, 0, 0, 0); d.dvw[2 * i + 1] = make_float4(0, 0, 0, 0);
+        v3 pos = mk3(p4);
+        q4 orn = mkq(d.orn[i]);
+        if (!tiled) {
+            v3 v = mk3(d.linvel[i]), w = mk3(d.angvel[i]);
+            integrate_body(v, w, pos, orn, mk3(d.dvw[2 * i]), mk3(d.dvw[2 * i + 1]), d.dt);
+            d.linvel[i] = f4(v, 0); d.angvel[i] = f4(w, 0);
+            d.pos[i] = f4(pos, p4.w); d.orn[i] = f4(orn);
+            d.dvw[2 * i] = make_float4(0, 0, 0, 0); d.dvw[2 * i + 1] = make_float4(0, 0, 0, 0);
+        }
         if (refresh) {
             store_invIW(d, i, world_inertia(orn, load_m3(d.invI, i)), p4.w);
             int sk = shape_of(f);
@@ -1714,6 +1605,42 @@ B2D_D void position_solve(PBody &A, PBody &B, v3 J0, v3 J1, v3 J2, v3 J3, float 
     }
     max_error = fmaxf(fabsf(error), max_error);
 }
+// contact_constraint::solve_position (contact_constraint.cpp:58-90) of one contact point: refreshes its normal (pn) and
+// distance (pa.w, contact_constraint.cpp:72-76), then corrects a penetration.  Shared by k_island_tiles and k_position_df;
+// the latter stores the refreshed point through out_a / out_n before the correction, so fewer registers stay live across it.
+B2D_D void contact_point_position(PBody &A, PBody &B, float4 &pa, const float4 &pb, float4 &pn, const float4 &pl, float &max_error,
+                                  float4 *out_a = nullptr, float4 *out_n = nullptr) {
+    v3 pAw = to_world(mk3(pa), A.pos, A.orn), pBw = to_world(mk3(pb), B.pos, B.orn);
+    unsigned att = __float_as_uint(pl.w) & 3u;
+    v3 normal = mk3(pn);
+    if (att == ATT_A) normal = rotate(A.orn, mk3(pl)); else if (att == ATT_B) normal = rotate(B.orn, mk3(pl));
+    float dist = dot(pAw - pBw, normal);
+    v3 rA = pAw - A.pos, rB = pBw - B.pos;
+    pn = f4(normal, pn.w); pa = f4(mk3(pa), dist);
+    if (out_n) { *out_n = pn; *out_a = pa; }
+    if (dist > -EPS) return;
+    position_solve(A, B, normal, cross(rA, normal), -normal, -cross(rB, normal), -dist, max_error);
+}
+// hinge_constraint::solve_position, hinge_constraint.cpp:180-213; returns the max error.  Shared by k_island_tiles and
+// k_position_df.
+B2D_D float hinge_position(PBody &A, PBody &B, v3 fA0, v3 fB0, v3 pvA, v3 pvB) {
+    float max_error = 0.0f;
+    v3 axisA = rotate(A.orn, fA0), axisB = rotate(B.orn, fB0);
+    v3 p, q; plane_space(axisA, p, q);
+    v3 u = cross(axisA, axisB);
+    const v3 z = mk3(0, 0, 0);
+    { float e = dot(u, p); if (fabsf(e) > EPS) position_solve(A, B, z, p, z, -p, e, max_error); }
+    { float e = dot(u, q); if (fabsf(e) > EPS) position_solve(A, B, z, q, z, -q, e, max_error); }
+    v3 pivotA = to_world(pvA, A.pos, A.orn), pivotB = to_world(pvB, B.pos, B.orn);
+    v3 dir = pivotA - pivotB;
+    float e = length(dir);
+    if (e > EPS) {
+        dir /= e;
+        v3 rA = pivotA - A.pos, rB = pivotB - B.pos;
+        position_solve(A, B, dir, cross(rA, dir), -dir, -cross(rB, dir), -e, max_error);
+    }
+    return max_error;
+}
 // Per-island max error, aggregated per warp first: in a pile every lane belongs to the same island and one atomic per
 // lane on a single address serialises the whole pass at the L2 atomic unit (0.9 ms per step at 262k bodies).
 B2D_D void island_error_max(const Dev &d, uint32_t isl, float err) {
@@ -1732,8 +1659,11 @@ B2D_D void tile_error_max(uint32_t *s_err, uint32_t islot, float err) { if (err 
 // tiled islands in ONE kernel: a tile's bodies, joints and manifolds are loaded once and their rows computed on chip, the
 // velocity iterations run, the bodies are integrated
 // where they sit (shared memory), the impulses go straight to the warm-start cache, the position iterations run on
-// the same records, and positions / orientations / velocities are written once.  Same arithmetic in the same order as
-// the separate kernels (k_prepare_contacts, k_prepare_hinges, k_integrate, k_store_impulses skip what this kernel has done).
+// the same records, and positions / orientations / velocities are written once.  One CTA per tile; thread t owns joint t
+// and manifold t of the tile for all iterations, and colours are separated by __syncthreads instead of tickets.  The row,
+// solve, integration and position functions are those of the separate kernels, called in the same order
+// (k_prepare_contacts, k_prepare_hinges, k_integrate, k_store_impulses skip what this kernel has done).  Without position
+// iterations the position loop does not run and the integrated pose is written back.
 // Two specialisations of one body (island_tiles<MAXP>), by the most contact points a manifold of the tile may have:
 // k_island_tiles (4) for the generic tiles, k_island_tiles_2p (2) for the two-point tiles, which keep less in registers
 // (ptxas: 40 B of spills at the 128-register cap instead of 280 B; under a 3-CTA bound, 80 registers, it spilled 646 B and
@@ -1848,19 +1778,18 @@ B2D_D void island_tiles(const Dev &d, int vel_iters, int pos_iters) {
         if (TWO && ch.z > 1) { s_p2[0] = b0; s_p2[TILE_CAP] = b1; s_p2[2 * TILE_CAP] = b2; s_p2[3 * TILE_CAP] = b3; s_p2[4 * TILE_CAP] = bim; }
         __syncthreads();
         const uint32_t nhc = s_ncol[0], ncc = s_ncol[1];
-        // ---- velocity iterations (as in k_solve_tiles)
+        // ---- velocity iterations
         for (int it = -1; it < vel_iters; ++it) {
             const bool warm = it < 0;
             for (uint32_t c = 0; c < nhc; ++c) {
                 if (hcol == c) {
                     const float4 r0 = s_hr[t], r1 = s_hr[TILE_CAP + t], r2 = s_hr[2 * TILE_CAP + t], r3 = s_hr[3 * TILE_CAP + t],
-                                 r4 = s_hr[4 * TILE_CAP + t], r5 = s_hr[5 * TILE_CAP + t], r6 = s_hr[6 * TILE_CAP + t];
-                    const float em[5] = {r0.w, r1.w, r2.w, r3.w, r4.x}, rhs[5] = {r4.y, r4.z, r4.w, r5.x, r5.y};
-                    float imp[5] = {r5.z, r5.w, r6.x, r6.y, r6.z};
+                                 r4 = s_hr[4 * TILE_CAP + t];
+                    float4 r5 = s_hr[5 * TILE_CAP + t], r6 = s_hr[6 * TILE_CAP + t];
                     VBody A, B; tf_load(s_body, hh.x, hh.w & 0xFFFFu, A); tf_load(s_body, hh.y, hh.w >> 16, B);
-                    hinge_solve(mk3(r0), mk3(r1), mk3(r2), mk3(r3), em, rhs, imp, A, B, warm);
+                    hinge_solve(r0, r1, r2, r3, r4, r5, r6, A, B, warm);
                     tf_store(s_body, hh.w & 0xFFFFu, A); tf_store(s_body, hh.w >> 16, B);
-                    if (!warm) { s_hr[5 * TILE_CAP + t] = make_float4(r5.x, r5.y, imp[0], imp[1]); s_hr[6 * TILE_CAP + t] = make_float4(imp[2], imp[3], imp[4], 0); }
+                    if (!warm) { s_hr[5 * TILE_CAP + t] = r5; s_hr[6 * TILE_CAP + t] = r6; }
                 }
                 __syncthreads();
             }
@@ -1946,11 +1875,9 @@ B2D_D void island_tiles(const Dev &d, int vel_iters, int pos_iters) {
         }
         // ---- integrate_velocities (k_integrate) for the tile's bodies; the records turn into position records
         if (t < nb) {
-            const float4 p4 = d.pos[mybody];
-            v3 v = mk3(d.linvel[mybody]), w = mk3(d.angvel[mybody]);
-            v += mk3(s_body[t]); w += mk3(s_body[TILE_CAP + t]);
-            v3 pos = mk3(p4); pos += v * d.dt;
-            const q4 orn = integrate(mkq(d.orn[mybody]), w, d.dt);
+            v3 v = mk3(d.linvel[mybody]), w = mk3(d.angvel[mybody]), pos = mk3(d.pos[mybody]);
+            q4 orn = mkq(d.orn[mybody]);
+            integrate_body(v, w, pos, orn, mk3(s_body[t]), mk3(s_body[TILE_CAP + t]), d.dt);
             d.linvel[mybody] = f4(v, 0); d.angvel[mybody] = f4(w, 0);
             s_body[t] = f4(pos, s_body[2 * TILE_CAP + t].w);     // inverse mass as the solvers see it
             s_body[TILE_CAP + t] = f4(orn);
@@ -1964,21 +1891,7 @@ B2D_D void island_tiles(const Dev &d, int vel_iters, int pos_iters) {
             for (uint32_t c = 0; c < nhc; ++c) {
                 if (hcol == c && !s_done[hisl]) {
                     PBody A, B; tq_load(s_body, hh.x, hh.w & 0xFFFFu, hpos, horn, A); tq_load(s_body, hh.y, hh.w >> 16, hpos, horn, B);
-                    float max_error = 0.0f;
-                    v3 axisA = rotate(A.orn, fA0), axisB = rotate(B.orn, fB0);
-                    v3 p, q; plane_space(axisA, p, q);
-                    v3 u = cross(axisA, axisB);
-                    const v3 z = mk3(0, 0, 0);
-                    { float e = dot(u, p); if (fabsf(e) > EPS) position_solve(A, B, z, p, z, -p, e, max_error); }
-                    { float e = dot(u, q); if (fabsf(e) > EPS) position_solve(A, B, z, q, z, -q, e, max_error); }
-                    v3 pivotA = to_world(pvA, A.pos, A.orn), pivotB = to_world(pvB, B.pos, B.orn);
-                    v3 dir = pivotA - pivotB;
-                    float e = length(dir);
-                    if (e > EPS) {
-                        dir /= e;
-                        v3 rA = pivotA - A.pos, rB = pivotB - B.pos;
-                        position_solve(A, B, dir, cross(rA, dir), -dir, -cross(rB, dir), -e, max_error);
-                    }
+                    const float max_error = hinge_position(A, B, fA0, fB0, pvA, pvB);
                     tq_store(s_body, hh.w & 0xFFFFu, A); tq_store(s_body, hh.w >> 16, B);
                     tile_error_max(s_err, hisl, max_error);
                 }
@@ -1988,25 +1901,14 @@ B2D_D void island_tiles(const Dev &d, int vel_iters, int pos_iters) {
                 if (ccol == c && !s_done[cisl]) {
                     PBody A, B; tq_load(s_body, ch.x, ch.w & 0xFFFFu, spos, sorn, A); tq_load(s_body, ch.y, ch.w >> 16, spos, sorn, B);
                     float max_error = 0.0f;
-                    auto point = [&](float4 &pa, const float4 &pb, float4 &pn, const float4 &pl) {
-                        v3 pAw = to_world(mk3(pa), A.pos, A.orn), pBw = to_world(mk3(pb), B.pos, B.orn);
-                        unsigned att = __float_as_uint(pl.w) & 3u;
-                        v3 normal = mk3(pn);
-                        if (att == ATT_A) normal = rotate(A.orn, mk3(pl)); else if (att == ATT_B) normal = rotate(B.orn, mk3(pl));
-                        float dist = dot(pAw - pBw, normal);
-                        v3 rA = pAw - A.pos, rB = pBw - B.pos;
-                        pn = f4(normal, pn.w); pa = f4(mk3(pa), dist);
-                        if (dist > -EPS) return;
-                        position_solve(A, B, normal, cross(rA, normal), -normal, -cross(rB, normal), -dist, max_error);
-                    };
                     if (!TWO) {
-                        point(a40, b40, n40, l40);
-                        if (ch.z > 1) point(a41, b41, n41, l41);
+                        contact_point_position(A, B, a40, b40, n40, l40, max_error);
+                        if (ch.z > 1) contact_point_position(A, B, a41, b41, n41, l41, max_error);
                     }
                     for (uint32_t s = TWO ? 0 : 2; s < ch.z; ++s) {
                         float4 *r = TWO ? s_pt + s * 4 * TILE_CAP : s_row + (s - 2) * 4 * TILE_CAP + t;
                         float4 pa = r[0], pn = r[2 * TILE_CAP];
-                        point(pa, r[TILE_CAP], pn, r[3 * TILE_CAP]);
+                        contact_point_position(A, B, pa, r[TILE_CAP], pn, r[3 * TILE_CAP], max_error);
                         r[0] = pa; r[2 * TILE_CAP] = pn;
                     }
                     tq_store(s_body, ch.w & 0xFFFFu, A); tq_store(s_body, ch.w >> 16, B);
@@ -2138,41 +2040,15 @@ B2D_D void contact_position_df(const Dev &d, uint4 hd, uint32_t m, uint2 tk2, ui
         for (uint32_t s = 0; s < n; ++s) {
             const size_t mi = (size_t)s * NM + m;
             if (s) { a4 = d.pA[mi]; b4 = d.pB[mi]; n4 = d.pN[mi]; l4 = d.pL[mi]; }
-            v3 pAw = to_world(mk3(a4), A.pos, A.orn), pBw = to_world(mk3(b4), B.pos, B.orn);
-            unsigned att = __float_as_uint(l4.w) & 3u;
-            v3 normal = mk3(n4);
-            if (att == ATT_A) normal = rotate(A.orn, mk3(l4)); else if (att == ATT_B) normal = rotate(B.orn, mk3(l4));
-            float dist = dot(pAw - pBw, normal);
-            v3 rA = pAw - A.pos, rB = pBw - B.pos;
-            d.pN[mi] = f4(normal, n4.w); d.pA[mi] = f4(mk3(a4), dist);
-            if (dist > -EPS) continue;
-            position_solve(A, B, normal, cross(rA, normal), -normal, -cross(rB, normal), -dist, max_error);
+            contact_point_position(A, B, a4, b4, n4, l4, max_error, &d.pA[mi], &d.pN[mi]);
         }
         return max_error;
     });
 }
-// hinge_constraint::solve_position, hinge_constraint.cpp:180-213
 B2D_D void hinge_position_df(const Dev &d, uint4 hd, uint2 tk2, uint32_t isl, int it, uint32_t mask) {
     const uint32_t h = hd.z;
     const v3 fA0 = mk3(d.hfA0[h]), fB0 = mk3(d.hfB0[h]), pvA = mk3(d.hpivA[h]), pvB = mk3(d.hpivB[h]);
-    position_chunk_df(d, hd.x, hd.y, tk2, isl, it, mask, [&](PBody &A, PBody &B) {
-        float max_error = 0.0f;
-        v3 axisA = rotate(A.orn, fA0), axisB = rotate(B.orn, fB0);
-        v3 p, q; plane_space(axisA, p, q);
-        v3 u = cross(axisA, axisB);
-        const v3 z = mk3(0, 0, 0);
-        { float e = dot(u, p); if (fabsf(e) > EPS) position_solve(A, B, z, p, z, -p, e, max_error); }
-        { float e = dot(u, q); if (fabsf(e) > EPS) position_solve(A, B, z, q, z, -q, e, max_error); }
-        v3 pivotA = to_world(pvA, A.pos, A.orn), pivotB = to_world(pvB, B.pos, B.orn);
-        v3 dir = pivotA - pivotB;
-        float e = length(dir);
-        if (e > EPS) {
-            dir /= e;
-            v3 rA = pivotA - A.pos, rB = pivotB - B.pos;
-            position_solve(A, B, dir, cross(rA, dir), -dir, -cross(rB, dir), -e, max_error);
-        }
-        return max_error;
-    });
+    position_chunk_df(d, hd.x, hd.y, tk2, isl, it, mask, [&](PBody &A, PBody &B) { return hinge_position(A, B, fA0, fB0, pvA, pvB); });
 }
 __global__ void __launch_bounds__(B2D_POS_THREADS, B2D_POS_MIN_BLOCKS) k_position_df(Dev d, int iters) {
     __shared__ uint32_t s_coff[MAX_COLORS + 2], s_cchunk[MAX_COLORS + 2], s_hoff[MAX_COLORS + 2], s_hchunk[MAX_COLORS + 2];

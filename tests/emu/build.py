@@ -1,8 +1,8 @@
 """TEST INFRASTRUCTURE.  Builds tests/emu/_build/libb2d_emu.so: the library's CUDA sources compiled for the CPU emulation of
 tests/emu/include/cuda_runtime.h.  The sources are used as they are except for what C++ cannot parse:
-  * kernel<<<grid, block, smem, stream>>>(args)  ->  EMU_LAUNCH(kernel, grid, block, smem, stream, args)      (4 sites)
+  * kernel<<<grid, block, smem, stream>>>(args)  ->  EMU_LAUNCH(kernel, grid, block, smem, stream, args)      (5 sites)
   * cudaLaunchCooperativeKernel(...)             ->  the same kernel on ONE block                             (1 site)
-  * extern __shared__ T name[];                  ->  T *name = emu::dynamic_smem()                            (2 sites)
+  * extern __shared__ T name[];                  ->  T *name = emu::dynamic_smem()                            (1 site)
   * the seven inline-PTX lines (acquire / relaxed polls, fences, prefetch, register pinning) -> plain loads / stores / no-ops,
     every poll yielding to the other fibers.
     python tests/emu/build.py        # g++ only, ~1 minute

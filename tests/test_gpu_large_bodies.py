@@ -103,7 +103,8 @@ def test_large_dynamic_bodies_lockstep(gpu, E, O, name):
 
 
 def test_large_dynamic_bodies_without_position_iterations(gpu, E, O):
-    """k_solve_tiles (no position iterations) instead of k_island_tiles."""
+    """The tile kernel without position iterations: it writes back the integrated pose and k_integrate refreshes the
+    tiled bodies' inertia and AABB."""
     for name in L.SCENES:
         scene = L.SCENES[name](E)
         assert_large(scene)

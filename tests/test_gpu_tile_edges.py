@@ -7,7 +7,7 @@ several position iterations next to one that stops after the first in the same t
 generic islands in root order.
 
 Every step of every scene, in three modes (plain launches, CUDA graphs with rebuild reuse, dataflow only) and at three
-iteration settings ((1, 0) runs k_solve_tiles): the packing against the restatement, the oracle lock step of
+iteration settings ((1, 0): the tile kernel without position iterations): the packing against the restatement, the oracle lock step of
 tests/emu/lockstep.py, and the three modes bit-identical to each other.  Also runs against the CPU emulation
 (B2D_EMU=1), which has no graphs and runs fewer steps."""
 import os
