@@ -1077,19 +1077,22 @@ B2D_D float rel_speed(v3 J0, v3 J1, v3 J2, v3 J3, v3 vA, v3 wA, v3 vB, v3 wB) {
 // contact_constraint::prepare (contact_constraint.cpp:15-56) + prepare_row of contact point slot mi: r0 = normal | rhs,
 // r1 = rA | eff_mass, r2 = rB | friction, r3 = eff_mass t0, t1, rhs t0, t1, im = warm-start impulses (n, t0, t1).
 // Row storage keeps (n, rA, rB) and rebuilds the Jacobian in registers: 84 B/point instead of the reference's 312 B
-// (constraint_row + _friction).  Shared by k_prepare_contacts and k_island_tiles, so both produce the same bits.
+// (constraint_row + _friction).  Shared by k_prepare_contacts, k_island_tiles and the restitution solver, so all produce
+// the same bits.  `restitution`: the rows of the restitution solver's groups (constraint_row_options{}, restitution_solver.cpp:
+// 146-310): no penetration error, the point's restitution always applied, no warm start.
 B2D_D void contact_point_rows(const Dev &d, size_t mi, const SBody &A, const SBody &B, v3 posA, q4 ornA, v3 posB, q4 ornB,
-                              float4 &r0, float4 &r1, float4 &r2, float4 &r3, float4 &imp) {
-    float4 a4 = d.pA[mi], b4 = d.pB[mi], n4 = d.pN[mi], im = d.pI[mi];
+                              float4 &r0, float4 &r1, float4 &r2, float4 &r3, float4 &imp, bool restitution = false) {
+    float4 a4 = d.pA[mi], b4 = d.pB[mi], n4 = d.pN[mi], im = restitution ? make_float4(0, 0, 0, 0) : d.pI[mi];
     v3 normal = mk3(n4);
     v3 pAw = to_world(mk3(a4), posA, ornA), pBw = to_world(mk3(b4), posB, ornB);
     v3 rA = pAw - posA, rB = pBw - posB;
     v3 J1 = cross(rA, normal), J2 = -normal, J3 = -cross(rB, normal);
     float em = eff_mass(normal, J1, J2, J3, A, B);
     float error = 0.0f;
-    if (a4.w > 0) error = a4.w / d.dt;
+    if (!restitution && a4.w > 0) error = a4.w / d.dt;
     float relvel = rel_speed(normal, J1, J2, J3, A.v, A.w, B.v, B.w);
-    float rhs = -(error * 0.2f + relvel * (1.0f + (d.rest_iters ? 0.0f : n4.w)));     // solver.cpp:217-236
+    // solver.cpp:217-236: with the restitution solver on, the ordinary rows carry no restitution
+    float rhs = -(error * 0.2f + relvel * (1.0f + (restitution ? n4.w : (d.rest_iters ? 0.0f : n4.w))));
     v3 t, u; plane_space(normal, t, u);
     v3 T1 = cross(rA, t), T2 = -t, T3 = -cross(rB, t);
     v3 U1 = cross(rA, u), U2 = -u, U3 = -cross(rB, u);
@@ -1129,6 +1132,48 @@ B2D_D void hinge_rows(const Dev &d, uint32_t h, const SBody &A, const SBody &B, 
     R[6 * stride] = make_float4(imp[2], imp[3], imp[4], 0);
 }
 
+// Row header of a sorted constraint (Dev::hdr / hhdr): the tags of bodies a and b, the point count or hinge id, and the
+// bodies' slots in an island tile.  A body tag is the body id, with the top bit set for a body the solver does not move.
+B2D_D uint32_t body_tag(uint32_t id, const SBody &b) { return id | (b.proc ? 0u : 0x80000000u); }
+B2D_D uint32_t tag_id(uint32_t tag) { return tag & 0x7FFFFFFFu; }
+B2D_D bool tag_proc(uint32_t tag) { return !(tag >> 31); }
+B2D_D uint32_t slot_pair(uint32_t sa, uint32_t sb) { return sa | (sb << 16); }
+B2D_D uint32_t slot_a(uint32_t pair) { return pair & 0xFFFFu; }
+B2D_D uint32_t slot_b(uint32_t pair) { return pair >> 16; }
+// island label of a constraint between bodies a and b (the dynamic one's)
+B2D_D uint32_t island_of(const Dev &d, uint32_t a, uint32_t b) { uint32_t l = d.parent[a]; return l != 0xFFFFFFFFu ? l : d.parent[b]; }
+
+// Dataflow tickets (k_solve_df, k_position_df): per body side of a constraint, the word S | base << 8 | k << 16.  Per
+// iteration a body sees its hinges (by colour), then its contact normals, then the friction pairs: S = its hinges + 2 x its
+// manifolds, base = the rank of this constraint's first pass in that sequence, k = its manifolds (a friction pass comes k
+// after its normal pass).  Colours are unique per body, so a rank is a popcount.
+B2D_D uint32_t ticket_word(uint32_t S, uint32_t base, uint32_t k) { return S | (base << 8) | (k << 16); }
+B2D_D uint2 constraint_tickets(const Dev &d, uint2 pr, uint32_t col, bool hinge) {
+    const unsigned long long below = (1ULL << col) - 1ULL;
+    uint32_t t[2];
+    const uint32_t ids[2] = {pr.x, pr.y};
+    #pragma unroll
+    for (int k = 0; k < 2; ++k) {
+        unsigned long long bm = d.bmask[ids[k]], jm = d.jmask[ids[k]];
+        uint32_t kc = __popcll(bm), kh = __popcll(jm);
+        t[k] = ticket_word(kh + 2 * kc, hinge ? __popcll(jm & below) : kh + __popcll(bm & below), kc);
+    }
+    return make_uint2(t[0], t[1]);
+}
+enum PassKind { PASS_HINGE, PASS_NORMAL, PASS_FRICTION, PASS_POSITION };
+struct Ticket { uint32_t ta, tb, mask; };
+// The tickets a pass waits for at its two bodies.  Velocity passes: pass = iteration + 1 (0 = warm start).  Position
+// passes: pass = position iteration, and as there are no friction passes a body sees S - k passes per iteration.
+B2D_D uint32_t ticket_at(uint32_t w, int pass, int kind) {
+    const uint32_t S = w & 0xFFu, base = (w >> 8) & 0xFFu, k = (w >> 16) & 0xFFu;
+    return (uint32_t)pass * (kind == PASS_POSITION ? S - k : S) + base + (kind == PASS_FRICTION ? k : 0u);
+}
+B2D_D Ticket ticket_of(uint2 tk, int pass, int kind, uint32_t mask) {
+    Ticket t;
+    t.mask = mask; t.ta = ticket_at(tk.x, pass, kind); t.tb = ticket_at(tk.y, pass, kind);
+    return t;
+}
+
 // Row preparation per sorted manifold; rows are written in colour order so the solve kernel streams them.
 // k_island_tiles prepares the tiled range [0, ntiled) itself and this kernel starts after it.
 __global__ void __launch_bounds__(256) k_prepare_contacts(Dev d) {
@@ -1142,23 +1187,10 @@ __global__ void __launch_bounds__(256) k_prepare_contacts(Dev d) {
         SBody A = solver_body(d, pr.x, fa), B = solver_body(d, pr.y, fb);
         v3 posA = mk3(d.pos[pr.x]), posB = mk3(d.pos[pr.y]);
         q4 ornA = mkq(d.orn[pr.x]), ornB = mkq(d.orn[pr.y]);
-        d.hdr[i] = make_uint4(pr.x | (A.proc ? 0u : 0x80000000u), pr.y | (B.proc ? 0u : 0x80000000u), npts,
-                              (A.proc ? d.bslot[pr.x] : SLOT_NONE) | ((B.proc ? d.bslot[pr.y] : SLOT_NONE) << 16));
-        {   // dataflow tickets: per iteration a body sees its hinges (by colour), then its contact normals, then the
-            // friction pairs; colours are unique per body, so the rank of this manifold is a popcount
-            const uint32_t col = (d.mstate[m] >> MS_COLOR_SHIFT) & 0xFFu;
-            const unsigned long long below = (1ULL << col) - 1ULL;
-            uint32_t t[2];
-            const uint32_t ids[2] = {pr.x, pr.y};
-            #pragma unroll
-            for (int k = 0; k < 2; ++k) {
-                unsigned long long bm = d.bmask[ids[k]], jm = d.jmask[ids[k]];
-                uint32_t kc = __popcll(bm), kh = __popcll(jm);
-                t[k] = (kh + 2 * kc) | ((kh + __popcll(bm & below)) << 8) | (kc << 16);
-            }
-            d.tkt[i] = make_uint2(t[0], t[1]);
-            { const uint32_t l = d.parent[pr.x]; d.pisl[i] = l != 0xFFFFFFFFu ? l : d.parent[pr.y]; }
-        }
+        d.hdr[i] = make_uint4(body_tag(pr.x, A), body_tag(pr.y, B), npts,
+                              slot_pair(A.proc ? d.bslot[pr.x] : SLOT_NONE, B.proc ? d.bslot[pr.y] : SLOT_NONE));
+        d.tkt[i] = constraint_tickets(d, pr, (d.mstate[m] >> MS_COLOR_SHIFT) & 0xFFu, false);
+        d.pisl[i] = island_of(d, pr.x, pr.y);
         for (uint32_t s = 0; s < npts; ++s) {
             const size_t ri = (size_t)s * d.NM + i;
             float4 r0, r1, r2, r3, im;
@@ -1180,20 +1212,10 @@ __global__ void k_prepare_hinges(Dev d) {
         v3 posA = mk3(d.pos[pr.x]), posB = mk3(d.pos[pr.y]);
         q4 ornA = mkq(d.orn[pr.x]), ornB = mkq(d.orn[pr.y]);
         hinge_rows(d, h, A, B, posA, ornA, posB, ornB, d.HR + 7 * (size_t)i, 1);
-        d.hhdr[i] = make_uint4(pr.x | (A.proc ? 0u : 0x80000000u), pr.y | (B.proc ? 0u : 0x80000000u), h,
-                               (A.proc ? d.bslot[pr.x] : SLOT_NONE) | ((B.proc ? d.bslot[pr.y] : SLOT_NONE) << 16));
-        {
-            const unsigned long long below = (1ULL << d.hcolor[h]) - 1ULL;
-            uint32_t t[2];
-            const uint32_t ids[2] = {pr.x, pr.y};
-            #pragma unroll
-            for (int k = 0; k < 2; ++k) {
-                unsigned long long bm = d.bmask[ids[k]], jm = d.jmask[ids[k]];
-                t[k] = (__popcll(jm) + 2 * __popcll(bm)) | (__popcll(jm & below) << 8) | (__popcll(bm) << 16);
-            }
-            d.htkt[i] = make_uint2(t[0], t[1]);
-            { const uint32_t l = d.parent[pr.x]; d.hisl[i] = l != 0xFFFFFFFFu ? l : d.parent[pr.y]; }
-        }
+        d.hhdr[i] = make_uint4(body_tag(pr.x, A), body_tag(pr.y, B), h,
+                               slot_pair(A.proc ? d.bslot[pr.x] : SLOT_NONE, B.proc ? d.bslot[pr.y] : SLOT_NONE));
+        d.htkt[i] = constraint_tickets(d, pr, d.hcolor[h], true);
+        d.hisl[i] = island_of(d, pr.x, pr.y);
     }
 }
 
@@ -1293,17 +1315,6 @@ B2D_D void hinge_solve(const float4 &r0, const float4 &r1, const float4 &r2, con
 // fixed sequence: iteration-major, then hinges / normals / frictions, then colour); afterwards it bumps them.  A pass
 // waits only for its own two predecessors (an L2 round trip) rather than for the slowest CTA of the whole grid.
 B2D_D void fence_gpu() { asm volatile("fence.acq_rel.gpu;" ::: "memory"); }
-struct Ticket { uint32_t ta, tb, mask; };
-// pass = iteration + 1 (0 = warm start); kind: 0 hinge, 1 contact normal, 2 friction
-B2D_D Ticket ticket_of(uint2 tk, int pass, int kind, uint32_t mask) {
-    Ticket t;
-    t.mask = mask;
-    const uint32_t SA = tk.x & 0xFFu, bA = (tk.x >> 8) & 0xFFu, kA = (tk.x >> 16) & 0xFFu;
-    const uint32_t SB = tk.y & 0xFFu, bB = (tk.y >> 8) & 0xFFu, kB = (tk.y >> 16) & 0xFFu;
-    t.ta = (uint32_t)pass * SA + bA + (kind == 2 ? kA : 0u);
-    t.tb = (uint32_t)pass * SB + bB + (kind == 2 ? kB : 0u);
-    return t;
-}
 // ptxas recycles the unused lanes of a 128-bit load as scratch registers straight away, and the write-after-write hazard
 // then parks the warp until the load has landed -- in front of the ticket poll.  keep() pins such a lane as live up to
 // the point where the rest of the vector is consumed.
@@ -1326,7 +1337,7 @@ B2D_D void st_volatile4(float4 *p, float4 v) {
 }
 // everything of a body that does not change during the solve
 B2D_D void vb_static(const Dev &d, uint32_t tag, VBody &b) {
-    b.proc = !(tag & 0x80000000u); b.id = tag & 0x7FFFFFFFu;
+    b.proc = tag_proc(tag); b.id = tag_id(tag);
     b.dv = mk3(0, 0, 0); b.dw = mk3(0, 0, 0);
     if (b.proc) {
         float4 r0 = d.invIW[3 * b.id], r1 = d.invIW[3 * b.id + 1], r2 = d.invIW[3 * b.id + 2];
@@ -1338,11 +1349,12 @@ B2D_D bool vb_try(const Dev &d, VBody &b, uint32_t expect) {
     b.dv = mk3(a); b.dw = mk3(w);
     return __float_as_uint(a.w) == expect && __float_as_uint(w.w) == expect;
 }
-// Lanes of a chunk become ready one by one; each lane solves as soon as ITS two bodies carry the expected tickets
-// (the ready subset runs the solve converged, the rest keep polling), so one late predecessor delays one constraint
-// and not the 31 others that happen to share its warp.
 B2D_D bool acquire_try(const Dev &d, const Ticket &t, VBody &A, VBody &B) {
     return (!A.proc || vb_try(d, A, t.ta)) & (!B.proc || vb_try(d, B, t.tb));
+}
+B2D_D void bodies_publish(const Dev &d, const Ticket &t, const VBody &A, const VBody &B) {
+    if (A.proc) { st_volatile4(&d.dvw[2 * A.id], f4(A.dv, __uint_as_float(t.ta + 1))); st_volatile4(&d.dvw[2 * A.id + 1], f4(A.dw, __uint_as_float(t.ta + 1))); }
+    if (B.proc) { st_volatile4(&d.dvw[2 * B.id], f4(B.dv, __uint_as_float(t.tb + 1))); st_volatile4(&d.dvw[2 * B.id + 1], f4(B.dw, __uint_as_float(t.tb + 1))); }
 }
 B2D_D bool acquire_more(const Dev &d, const Ticket &t, bool pending, bool progressed, uint32_t &spins) {
     if (!__any_sync(t.mask, pending)) return false;
@@ -1352,101 +1364,82 @@ B2D_D bool acquire_more(const Dev &d, const Ticket &t, bool pending, bool progre
     }
     return true;
 }
-B2D_D void bodies_publish(const Dev &d, const Ticket &t, const VBody &A, const VBody &B) {
-    if (A.proc) { st_volatile4(&d.dvw[2 * A.id], f4(A.dv, __uint_as_float(t.ta + 1))); st_volatile4(&d.dvw[2 * A.id + 1], f4(A.dw, __uint_as_float(t.ta + 1))); }
-    if (B.proc) { st_volatile4(&d.dvw[2 * B.id], f4(B.dv, __uint_as_float(t.tb + 1))); st_volatile4(&d.dvw[2 * B.id + 1], f4(B.dw, __uint_as_float(t.tb + 1))); }
+// One pass of a constraint, for every lane of t.mask: poll() fetches the two bodies' records and says whether both carry
+// the tickets of t; then work() runs and publish() writes the records with the next tickets.  Lanes of a chunk become
+// ready one by one; each lane solves as soon as ITS two bodies carry the expected tickets (the ready subset runs the
+// solve converged, the rest keep polling), so one late predecessor delays one constraint and not the 31 others that
+// happen to share its warp.
+template<typename Poll, typename Work, typename Publish>
+B2D_D void ticket_wait(const Dev &d, const Ticket &t, Poll poll, Work work, Publish publish) {
+    bool pending = true; uint32_t spins = 0;
+    do {
+        const bool ok = pending && poll();
+        if (ok) {
+            work();
+            publish();
+            pending = false;
+        }
+        if (!acquire_more(d, t, pending, ok, spins)) break;
+    } while (true);
 }
 
 B2D_D void hinge_pass(const Dev &d, uint32_t i, bool warm, int pass, uint32_t mask) {
     uint4 hd = d.hhdr[i];
     float4 *R = d.HR + 7 * (size_t)i;
     float4 r0 = R[0], r1 = R[1], r2 = R[2], r3 = R[3], r4 = R[4], r5 = R[5], r6 = R[6];
-    const Ticket tk = ticket_of(d.htkt[i], pass, 0, mask);
+    const Ticket tk = ticket_of(d.htkt[i], pass, PASS_HINGE, mask);
     VBody A, B; vb_static(d, hd.x, A); vb_static(d, hd.y, B);
-    bool pending = true; uint32_t spins = 0;
-    do {
-    const bool ok = pending && acquire_try(d, tk, A, B);
-    if (ok) {
-    hinge_solve(r0, r1, r2, r3, r4, r5, r6, A, B, warm);
-    bodies_publish(d, tk, A, B);
-    if (!warm) { R[5] = r5; R[6] = r6; }
-    pending = false;
-    }
-    if (!acquire_more(d, tk, pending, ok, spins)) break;
-    } while (true);
+    ticket_wait(d, tk, [&] { return acquire_try(d, tk, A, B); },
+                [&] { hinge_solve(r0, r1, r2, r3, r4, r5, r6, A, B, warm); },
+                [&] { bodies_publish(d, tk, A, B); if (!warm) { R[5] = r5; R[6] = r6; } });
 }
 
-// Row loads are issued ahead of the dependent computation: slots 0 and 1 before the ticket wait / body loads,
-// slots 2 and 3 (box faces, ~15 % of manifolds) into the registers freed by slots 0 and 1 while those are being
-// solved.  Impulses are private to the owning thread and stored as soon as they are final.
-B2D_D void prefetch_L2(const void *p) { asm volatile("prefetch.global.L2 [%0];" :: "l"(p)); }
-struct NRow { float4 r0, r1, r2, im; };
+// The rows of one contact point for a normal pass (NRow) or a friction pass (FRow): load() streams them in, pin() keeps
+// the lanes the solve does not read, solve() runs the row and stores its impulses.
 #ifndef B2D_ROW_LD
 #define B2D_ROW_LD(p) __ldcs(p)       // rows stream past L1 (evict-first): the per-body data keeps it
 #endif
-B2D_D NRow load_nrow(const Dev &d, size_t ri) { NRow r; r.r0 = B2D_ROW_LD(&d.R0[ri]); r.r1 = B2D_ROW_LD(&d.R1[ri]); r.r2 = B2D_ROW_LD(&d.R2[ri]); r.im = B2D_ROW_LD(&d.IMP[ri]); return r; }
-B2D_D void solve_nrow(const Dev &d, NRow &r, size_t ri, VBody &A, VBody &B, bool warm) {
-    nrow_solve(r.r0, r.r1, r.r2, r.im, A, B, warm);
-    if (!warm) d.IMP[ri] = r.im;
-}
-B2D_D void normal_pass(const Dev &d, uint32_t i, const uint4 hd, const uint2 tk2, bool warm, int pass, uint32_t mask) {
-    const Ticket tk = ticket_of(tk2, pass, 1, mask);
+struct NRow {
+    static constexpr int KIND = PASS_NORMAL;
+    float4 r0, r1, r2, im;
+    B2D_D void load(const Dev &d, size_t ri) { r0 = B2D_ROW_LD(&d.R0[ri]); r1 = B2D_ROW_LD(&d.R1[ri]); r2 = B2D_ROW_LD(&d.R2[ri]); im = B2D_ROW_LD(&d.IMP[ri]); }
+    B2D_D void pin() const { keep(r2.w); keep(im.y); keep(im.z); keep(im.w); }
+    B2D_D void solve(const Dev &d, size_t ri, VBody &A, VBody &B, bool warm) {
+        nrow_solve(r0, r1, r2, im, A, B, warm);
+        if (!warm) d.IMP[ri] = im;
+    }
+};
+struct FRow {
+    static constexpr int KIND = PASS_FRICTION;
+    float4 r0, r1, r2, r3, im;
+    B2D_D void load(const Dev &d, size_t ri) { r0 = B2D_ROW_LD(&d.R0[ri]); r1 = B2D_ROW_LD(&d.R1[ri]); r2 = B2D_ROW_LD(&d.R2[ri]); r3 = B2D_ROW_LD(&d.R3[ri]); im = B2D_ROW_LD(&d.IMP[ri]); }
+    B2D_D void pin() const { keep(r0.w); keep(r1.w); keep(im.w); }
+    B2D_D void solve(const Dev &d, size_t ri, VBody &A, VBody &B, bool warm) {
+        frow_solve(r0, r1, r2, r3, im, A, B, warm);
+        if (!warm) d.IMP[ri] = im;
+    }
+};
+// Row loads are issued ahead of the dependent computation: slots 0 and 1 before the ticket wait / body loads,
+// slots 2 and 3 (box faces, ~15 % of manifolds) into the registers freed by slots 0 and 1 while those are being
+// solved.  Impulses are private to the owning thread and stored as soon as they are final.
+template<typename Row>
+B2D_D void contact_pass(const Dev &d, uint32_t i, const uint4 hd, const uint2 tk2, bool warm, int pass, uint32_t mask) {
+    const Ticket tk = ticket_of(tk2, pass, Row::KIND, mask);
     const uint32_t n = hd.z;
     const size_t NM = d.NM;
-    NRow ra, rb;
-    ra = load_nrow(d, i);
-    rb = load_nrow(d, n > 1 ? NM + i : i);          // unconditional: a predicated load drags a zero-fill + WAW wait along
+    Row ra, rb;
+    ra.load(d, i);
+    rb.load(d, n > 1 ? NM + i : i);                 // unconditional: a predicated load drags a zero-fill + WAW wait along
     VBody A, B; vb_static(d, hd.x, A); vb_static(d, hd.y, B);
-    bool pending = true; uint32_t spins = 0;
-    do {
-    const bool ok = pending && acquire_try(d, tk, A, B);
-    if (ok) {
-    keep(A); keep(B); keep(hd.w); keep(ra.r2.w); keep(ra.im.y); keep(ra.im.z); keep(ra.im.w);
-    keep(rb.r2.w); keep(rb.im.y); keep(rb.im.z); keep(rb.im.w);
-    solve_nrow(d, ra, i, A, B, warm);
-    if (n > 2) ra = load_nrow(d, 2 * NM + i);
-    if (n > 1) solve_nrow(d, rb, NM + i, A, B, warm);
-    if (n > 3) rb = load_nrow(d, 3 * NM + i);
-    if (n > 2) solve_nrow(d, ra, 2 * NM + i, A, B, warm);
-    if (n > 3) solve_nrow(d, rb, 3 * NM + i, A, B, warm);
-    bodies_publish(d, tk, A, B);
-    pending = false;
-    }
-    if (!acquire_more(d, tk, pending, ok, spins)) break;
-    } while (true);
-}
-
-struct FRow { float4 r0, r1, r2, r3, im; };
-B2D_D FRow load_frow(const Dev &d, size_t ri) { FRow r; r.r0 = B2D_ROW_LD(&d.R0[ri]); r.r1 = B2D_ROW_LD(&d.R1[ri]); r.r2 = B2D_ROW_LD(&d.R2[ri]); r.r3 = B2D_ROW_LD(&d.R3[ri]); r.im = B2D_ROW_LD(&d.IMP[ri]); return r; }
-B2D_D void solve_frow(const Dev &d, FRow &r, size_t ri, VBody &A, VBody &B, bool warm) {
-    frow_solve(r.r0, r.r1, r.r2, r.r3, r.im, A, B, warm);
-    if (!warm) d.IMP[ri] = r.im;
-}
-B2D_D void friction_pass(const Dev &d, uint32_t i, const uint4 hd, const uint2 tk2, bool warm, int pass, uint32_t mask) {
-    const Ticket tk = ticket_of(tk2, pass, 2, mask);
-    const uint32_t n = hd.z;
-    const size_t NM = d.NM;
-    FRow ra, rb;
-    ra = load_frow(d, i);
-    rb = load_frow(d, n > 1 ? NM + i : i);
-    VBody A, B; vb_static(d, hd.x, A); vb_static(d, hd.y, B);
-    bool pending = true; uint32_t spins = 0;
-    do {
-    const bool ok = pending && acquire_try(d, tk, A, B);
-    if (ok) {
-    keep(A); keep(B); keep(hd.w); keep(ra.r0.w); keep(ra.r1.w); keep(ra.im.w);
-    keep(rb.r0.w); keep(rb.r1.w); keep(rb.im.w);
-    solve_frow(d, ra, i, A, B, warm);
-    if (n > 2) ra = load_frow(d, 2 * NM + i);
-    if (n > 1) solve_frow(d, rb, NM + i, A, B, warm);
-    if (n > 3) rb = load_frow(d, 3 * NM + i);
-    if (n > 2) solve_frow(d, ra, 2 * NM + i, A, B, warm);
-    if (n > 3) solve_frow(d, rb, 3 * NM + i, A, B, warm);
-    bodies_publish(d, tk, A, B);
-    pending = false;
-    }
-    if (!acquire_more(d, tk, pending, ok, spins)) break;
-    } while (true);
+    ticket_wait(d, tk, [&] { return acquire_try(d, tk, A, B); }, [&] {
+        keep(A); keep(B); keep(hd.w); ra.pin(); rb.pin();
+        ra.solve(d, i, A, B, warm);
+        if (n > 2) ra.load(d, 2 * NM + i);
+        if (n > 1) rb.solve(d, NM + i, A, B, warm);
+        if (n > 3) rb.load(d, 3 * NM + i);
+        if (n > 2) ra.solve(d, 2 * NM + i, A, B, warm);
+        if (n > 3) rb.solve(d, 3 * NM + i, A, B, warm);
+    }, [&] { bodies_publish(d, tk, A, B); });
 }
 
 // Work is dealt to warps in 32-constraint chunks that never span two colours (so lanes of a warp never wait on each
@@ -1458,56 +1451,90 @@ B2D_D uint32_t chunk_index(const uint32_t *chunk, const uint32_t *off, uint32_t 
     while (j >= chunk[col + 1]) ++col;
     return off[col] + (j - chunk[col]) * 32u;
 }
+// colour tables of the dataflow kernels, in shared memory: every chunk walk reads them, and a global read costs an L2 round trip
+struct ChunkTables { uint32_t coff[MAX_COLORS + 2], cchunk[MAX_COLORS + 2], hoff[MAX_COLORS + 2], hchunk[MAX_COLORS + 2]; };
+// A warp's walk over its hinge chunks and its contact chunks.  The head of the warp's NEXT contact chunk (Head::fetch:
+// header and ticket words, the same for every pass and both row types) is fetched one chunk ahead into registers, so a
+// chunk starts polling its bodies without first waiting for its own header.
+template<typename Head>
+struct ChunkWalk {
+    const ChunkTables &s;
+    uint32_t lane, wid, nw, hchunks, cchunks;
+    uint32_t ncol = 0, ni = 0; bool nact = false; Head next{};
+    B2D_D ChunkWalk(const Dev &d, ChunkTables &t) : s(t) {
+        const Counters &c = *d.cnt;
+        if (threadIdx.x < MAX_COLORS + 2) {
+            t.coff[threadIdx.x] = c.coff[threadIdx.x]; t.cchunk[threadIdx.x] = c.cchunk[threadIdx.x];
+            t.hoff[threadIdx.x] = c.hoff[threadIdx.x]; t.hchunk[threadIdx.x] = c.hchunk[threadIdx.x];
+        }
+        const uint32_t nc = c.ncolors, nh = c.nhcolors;
+        __syncthreads();
+        lane = threadIdx.x & 31u;
+        wid = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; nw = (gridDim.x * blockDim.x) >> 5;
+        hchunks = s.hchunk[nh]; cchunks = s.cchunk[nc];
+    }
+    // the head of the warp's first contact chunk
+    B2D_D void start(const Dev &d) {
+        if (wid < cchunks) {
+            ni = chunk_index(s.cchunk, s.coff, wid, ncol) + lane; nact = ni < s.coff[ncol + 1];
+            if (nact) next.fetch(d, ni);
+        }
+    }
+    // per_lane(i, mask) for each sorted hinge i of the warp's hinge chunks
+    template<typename PerLane>
+    B2D_D void hinges(PerLane per_lane) {
+        uint32_t col = 0;
+        for (uint32_t j = wid; j < hchunks; j += nw) {
+            const uint32_t i = chunk_index(s.hchunk, s.hoff, j, col) + lane;
+            const bool act = i < s.hoff[col + 1];
+            const uint32_t mask = __ballot_sync(0xffffffffu, act);
+            if (act) per_lane(i, mask);
+        }
+    }
+    // per_lane(i, head, mask) for each sorted manifold i of the warp's contact chunks; ahead(i, wrapped) runs once the
+    // head of manifold i of the next chunk has been fetched (wrapped: that chunk is the warp's first, of the next pass)
+    template<typename Ahead, typename PerLane>
+    B2D_D void contacts(const Dev &d, Ahead ahead, PerLane per_lane) {
+        for (uint32_t j = wid; j < cchunks; j += nw) {
+            const uint32_t i = ni; const bool act = nact; const Head head = next;
+            uint32_t jn = j + nw;
+            if (jn >= cchunks) { jn = wid; ncol = 0; }
+            ni = chunk_index(s.cchunk, s.coff, jn, ncol) + lane; nact = ni < s.coff[ncol + 1];
+            if (nact) {
+                next.fetch(d, ni);
+                ahead(ni, jn == wid);
+            }
+            const uint32_t mask = __ballot_sync(0xffffffffu, act);
+            if (act) per_lane(i, head, mask);
+        }
+    }
+};
+struct ContactHead {
+    uint4 hd; uint2 tk;
+    B2D_D void fetch(const Dev &d, uint32_t i) { hd = d.hdr[i]; tk = d.tkt[i]; }
+};
+B2D_D void prefetch_L2(const void *p) { asm volatile("prefetch.global.L2 [%0];" :: "l"(p)); }
 #ifndef B2D_SOLVE_THREADS
 #define B2D_SOLVE_THREADS 256
 #endif
 __global__ void __launch_bounds__(B2D_SOLVE_THREADS, 2) k_solve_df(Dev d, int iters) {
-    // colour tables live in shared memory: every chunk walk reads them, and a global read costs an L2 round trip
-    __shared__ uint32_t s_coff[MAX_COLORS + 2], s_cchunk[MAX_COLORS + 2], s_hoff[MAX_COLORS + 2], s_hchunk[MAX_COLORS + 2];
-    const Counters &c = *d.cnt;
-    if (threadIdx.x < MAX_COLORS + 2) {
-        s_coff[threadIdx.x] = c.coff[threadIdx.x]; s_cchunk[threadIdx.x] = c.cchunk[threadIdx.x];
-        s_hoff[threadIdx.x] = c.hoff[threadIdx.x]; s_hchunk[threadIdx.x] = c.hchunk[threadIdx.x];
-    }
-    const uint32_t nc = c.ncolors, nh = c.nhcolors;
-    __syncthreads();
-    const uint32_t lane = threadIdx.x & 31u;
-    const uint32_t wid = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
-    const uint32_t hchunks = s_hchunk[nh], cchunks = s_cchunk[nc];
-    if (hchunks + cchunks == 0) return;
-    // The header and ticket words of this warp's NEXT contact chunk are fetched one chunk ahead into registers (they
-    // are the same for every pass and both row types), so a chunk starts polling its bodies without first waiting for
-    // its own header; the rows of the next chunk are pulled towards L2 at the same time.
-    uint32_t ncol = 0, ni = 0; bool nact = false; uint4 nhd = make_uint4(0, 0, 0, 0); uint2 ntk = make_uint2(0, 0);
-    if (wid < cchunks) {
-        ni = chunk_index(s_cchunk, s_coff, wid, ncol) + lane; nact = ni < s_coff[ncol + 1];
-        if (nact) { nhd = d.hdr[ni]; ntk = d.tkt[ni]; }
-    }
+    __shared__ ChunkTables tables;
+    ChunkWalk<ContactHead> walk(d, tables);
+    if (walk.hchunks + walk.cchunks == 0) return;
+    walk.start(d);
     for (int it = -1; it < iters; ++it) {
         const bool warm = it < 0;
         const int pass = it + 1;
-        { uint32_t col = 0;
-          for (uint32_t j = wid; j < hchunks; j += nw) {
-              const uint32_t i = chunk_index(s_hchunk, s_hoff, j, col) + lane;
-              const bool act = i < s_hoff[col + 1];
-              const uint32_t mask = __ballot_sync(0xffffffffu, act);
-              if (act) hinge_pass(d, i, warm, pass, mask);
-          } }
+        walk.hinges([&](uint32_t i, uint32_t mask) { hinge_pass(d, i, warm, pass, mask); });
         #pragma unroll 1
-        for (int kind = 1; kind <= 2; ++kind) {
-            for (uint32_t j = wid; j < cchunks; j += nw) {
-                const uint32_t i = ni; const bool act = nact; const uint4 hd = nhd; const uint2 tk2 = ntk;
-                uint32_t jn = j + nw;
-                if (jn >= cchunks) { jn = wid; ncol = 0; }
-                ni = chunk_index(s_cchunk, s_coff, jn, ncol) + lane; nact = ni < s_coff[ncol + 1];
-                if (nact) {
-                    nhd = d.hdr[ni]; ntk = d.tkt[ni];
-                    prefetch_L2(&d.R0[ni]); prefetch_L2(&d.R1[ni]); prefetch_L2(&d.R2[ni]); prefetch_L2(&d.IMP[ni]);
-                    if (kind == 2 || jn == wid) prefetch_L2(&d.R3[ni]);
-                }
-                const uint32_t mask = __ballot_sync(0xffffffffu, act);
-                if (act) { if (kind == 1) normal_pass(d, i, hd, tk2, warm, pass, mask); else friction_pass(d, i, hd, tk2, warm, pass, mask); }
-            }
+        for (int kind = PASS_NORMAL; kind <= PASS_FRICTION; ++kind) {
+            walk.contacts(d, [&](uint32_t ni, bool wrapped) {      // the rows of the next chunk are pulled towards L2
+                prefetch_L2(&d.R0[ni]); prefetch_L2(&d.R1[ni]); prefetch_L2(&d.R2[ni]); prefetch_L2(&d.IMP[ni]);
+                if (kind == PASS_FRICTION || wrapped) prefetch_L2(&d.R3[ni]);
+            }, [&](uint32_t i, const ContactHead &h, uint32_t mask) {
+                if (kind == PASS_NORMAL) contact_pass<NRow>(d, i, h.hd, h.tk, warm, pass, mask);
+                else contact_pass<FRow>(d, i, h.hd, h.tk, warm, pass, mask);
+            });
         }
     }
 }
@@ -1540,6 +1567,13 @@ B2D_D void integrate_body(v3 &v, v3 &w, v3 &pos, q4 &orn, v3 dv, v3 dw, float dt
     pos += v * dt;
     orn = integrate(orn, w, dt);
 }
+// update_aabbs + update_inertias (solver.cpp:453-465) of body i at (pos, orn): the AABB of a shaped body, the world-space
+// inverse inertia of a dynamic one
+B2D_D void refresh_body(const Dev &d, uint32_t i, uint32_t f, v3 pos, q4 orn, float inv_m) {
+    const int sk = shape_of(f);
+    if (sk != SH_NONE) { box3 bb = shape_aabb(sk, d.shp[i], pos, orn); d.bbmin[i] = f4(bb.mn, 0); d.bbmax[i] = f4(bb.mx, 0); }
+    if (is_dynamic(f)) store_invIW(d, i, world_inertia(orn, load_m3(d.invI, i)), inv_m);
+}
 // integrate_velocities of the bodies outside the island tiles (k_island_tiles integrates its own); with refresh != 0
 // also update_aabbs + update_inertias (solver.cpp:453-465) of every dynamic body, tiled ones included, for when no
 // position iterations run in between.
@@ -1560,23 +1594,16 @@ __global__ void __launch_bounds__(256) k_integrate(Dev d, int refresh) {
             d.pos[i] = f4(pos, p4.w); d.orn[i] = f4(orn);
             d.dvw[2 * i] = make_float4(0, 0, 0, 0); d.dvw[2 * i + 1] = make_float4(0, 0, 0, 0);
         }
-        if (refresh) {
-            store_invIW(d, i, world_inertia(orn, load_m3(d.invI, i)), p4.w);
-            int sk = shape_of(f);
-            if (sk != SH_NONE) { box3 bb = shape_aabb(sk, d.shp[i], pos, orn); d.bbmin[i] = f4(bb.mn, 0); d.bbmax[i] = f4(bb.mx, 0); }
-        }
+        if (refresh) refresh_body(d, i, f, pos, orn, p4.w);
     }
 }
-// update_aabbs (dynamic + kinematic) and update_inertias (dynamic), solver.cpp:453-465
+// refresh_body of the dynamic and kinematic bodies after the position iterations
 __global__ void __launch_bounds__(256) k_finalize(Dev d) {
     GRID_STRIDE(i, d.nbodies) {
         uint32_t f = d.flags[i];
         if (kind_of(f) == 2u) continue;
         float4 p4 = d.pos[i];
-        v3 pos = mk3(p4); q4 orn = mkq(d.orn[i]);
-        int sk = shape_of(f);
-        if (sk != SH_NONE) { box3 bb = shape_aabb(sk, d.shp[i], pos, orn); d.bbmin[i] = f4(bb.mn, 0); d.bbmax[i] = f4(bb.mx, 0); }
-        if (is_dynamic(f)) store_invIW(d, i, world_inertia(orn, load_m3(d.invI, i)), p4.w);
+        refresh_body(d, i, f, mk3(p4), mkq(d.orn[i]), p4.w);
     }
 }
 
@@ -1649,8 +1676,8 @@ B2D_D void island_error_max(const Dev &d, uint32_t isl, float err) {
     const uint32_t m = __reduce_max_sync(grp, __float_as_uint(err));
     if ((threadIdx.x & 31u) == (uint32_t)(__ffs(grp) - 1) && m) atomicMax(&d.isl_err[isl], m);
 }
-B2D_D uint32_t island_of(const Dev &d, uint32_t a, uint32_t b) { uint32_t l = d.parent[a]; return l != 0xFFFFFFFFu ? l : d.parent[b]; }
-
+// the position iterations' early-out: an island whose max error fell below 0.005 is done (island_solver.cpp:538-543)
+B2D_D bool island_done(float max_error) { return max_error < 0.005f; }
 
 // per-island max error of a tile, kept at the shared-memory slot of the island's root body
 B2D_D void tile_error_max(uint32_t *s_err, uint32_t islot, float err) { if (err != 0.0f) atomicMax(&s_err[islot], __float_as_uint(err)); }
@@ -1690,7 +1717,7 @@ B2D_D void tile_solver_body(const Dev &d, const float4 *sb, uint32_t id, SBody &
     pos = mk3(sb[5 * TILE_CAP + slot]); orn = mkq(sb[6 * TILE_CAP + slot]);
 }
 B2D_D void tf_load(const float4 *sb, uint32_t tag, uint32_t slot, VBody &b) {           // velocity phase: SoA records
-    b.proc = !(tag & 0x80000000u); b.id = tag & 0x7FFFFFFFu;
+    b.proc = tag_proc(tag); b.id = tag_id(tag);
     if (b.proc) {
         const float4 a = sb[slot], w = sb[TILE_CAP + slot], r0 = sb[2 * TILE_CAP + slot], r1 = sb[3 * TILE_CAP + slot], r2 = sb[4 * TILE_CAP + slot];
         b.dv = mk3(a); b.dw = mk3(w); b.inv_m = r0.w; b.inv_I.r0 = mk3(r0); b.inv_I.r1 = mk3(r1); b.inv_I.r2 = mk3(r2);
@@ -1701,7 +1728,7 @@ B2D_D void tf_store(float4 *sb, uint32_t slot, const VBody &b) {
 }
 // position phase; a non-procedural partner (static / kinematic) is read from the thread's own copy
 B2D_D void tq_load(const float4 *sb, uint32_t tag, uint32_t slot, const float4 &spos, const float4 &sorn, PBody &b) {
-    b.id = tag & 0x7FFFFFFFu; b.proc = !(tag >> 31); b.fresh = false;
+    b.id = tag_id(tag); b.proc = tag_proc(tag); b.fresh = false;
     if (b.proc) {
         const float4 p = sb[slot];
         b.pos = mk3(p); b.inv_m = p.w; b.orn = mkq(sb[TILE_CAP + slot]);
@@ -1751,7 +1778,7 @@ B2D_D void island_tiles(const Dev &d, int vel_iters, int pos_iters) {
             SBody A, B; v3 posA, posB; q4 ornA, ornB; uint32_t sa, sb;
             tile_solver_body(d, s_body, pr.x, A, posA, ornA, sa); tile_solver_body(d, s_body, pr.y, B, posB, ornB, sb);
             hinge_rows(d, h, A, B, posA, ornA, posB, ornB, s_hr + t, TILE_CAP);
-            hh = make_uint4(pr.x | (A.proc ? 0u : 0x80000000u), pr.y | (B.proc ? 0u : 0x80000000u), h, sa | (sb << 16));
+            hh = make_uint4(body_tag(pr.x, A), body_tag(pr.y, B), h, slot_pair(sa, sb));
             hcol = d.hkey_s[hi] & 63u;
             atomicMax(&s_ncol[0], hcol + 1u);
         }
@@ -1763,7 +1790,7 @@ B2D_D void island_tiles(const Dev &d, int vel_iters, int pos_iters) {
             tile_solver_body(d, s_body, pr.x, A, posA, ornA, sa); tile_solver_body(d, s_body, pr.y, B, posB, ornB, sb);
             // a two-point tile holds no manifold with more points: one that gains a third point sets graph_changed
             // (k_np_merge) and the rebuild moves its island to a generic tile before the next solve
-            ch = make_uint4(pr.x | (A.proc ? 0u : 0x80000000u), pr.y | (B.proc ? 0u : 0x80000000u), TWO ? min(npts, 2u) : npts, sa | (sb << 16));
+            ch = make_uint4(body_tag(pr.x, A), body_tag(pr.y, B), TWO ? min(npts, 2u) : npts, slot_pair(sa, sb));
             contact_point_rows(d, m, A, B, posA, ornA, posB, ornB, a0, a1, a2, a3, aim);
             if (npts > 1) contact_point_rows(d, NM + m, A, B, posA, ornA, posB, ornB, b0, b1, b2, b3, bim);
             if (!TWO) for (uint32_t s = 2; s < npts; ++s) {
@@ -1786,16 +1813,16 @@ B2D_D void island_tiles(const Dev &d, int vel_iters, int pos_iters) {
                     const float4 r0 = s_hr[t], r1 = s_hr[TILE_CAP + t], r2 = s_hr[2 * TILE_CAP + t], r3 = s_hr[3 * TILE_CAP + t],
                                  r4 = s_hr[4 * TILE_CAP + t];
                     float4 r5 = s_hr[5 * TILE_CAP + t], r6 = s_hr[6 * TILE_CAP + t];
-                    VBody A, B; tf_load(s_body, hh.x, hh.w & 0xFFFFu, A); tf_load(s_body, hh.y, hh.w >> 16, B);
+                    VBody A, B; tf_load(s_body, hh.x, slot_a(hh.w), A); tf_load(s_body, hh.y, slot_b(hh.w), B);
                     hinge_solve(r0, r1, r2, r3, r4, r5, r6, A, B, warm);
-                    tf_store(s_body, hh.w & 0xFFFFu, A); tf_store(s_body, hh.w >> 16, B);
+                    tf_store(s_body, slot_a(hh.w), A); tf_store(s_body, slot_b(hh.w), B);
                     if (!warm) { s_hr[5 * TILE_CAP + t] = r5; s_hr[6 * TILE_CAP + t] = r6; }
                 }
                 __syncthreads();
             }
             for (uint32_t c = 0; c < ncc; ++c) {
                 if (ccol == c) {
-                    VBody A, B; tf_load(s_body, ch.x, ch.w & 0xFFFFu, A); tf_load(s_body, ch.y, ch.w >> 16, B);
+                    VBody A, B; tf_load(s_body, ch.x, slot_a(ch.w), A); tf_load(s_body, ch.y, slot_b(ch.w), B);
                     nrow_solve(a0, a1, a2, aim, A, B, warm);
                     if (TWO && ch.z > 1) {
                         float4 im = s_p2[4 * TILE_CAP];
@@ -1809,13 +1836,13 @@ B2D_D void island_tiles(const Dev &d, int vel_iters, int pos_iters) {
                         nrow_solve(r[0], r[TILE_CAP], r[2 * TILE_CAP], im, A, B, warm);
                         r[4 * TILE_CAP] = im;
                     }
-                    tf_store(s_body, ch.w & 0xFFFFu, A); tf_store(s_body, ch.w >> 16, B);
+                    tf_store(s_body, slot_a(ch.w), A); tf_store(s_body, slot_b(ch.w), B);
                 }
                 __syncthreads();
             }
             for (uint32_t c = 0; c < ncc; ++c) {
                 if (ccol == c) {
-                    VBody A, B; tf_load(s_body, ch.x, ch.w & 0xFFFFu, A); tf_load(s_body, ch.y, ch.w >> 16, B);
+                    VBody A, B; tf_load(s_body, ch.x, slot_a(ch.w), A); tf_load(s_body, ch.y, slot_b(ch.w), B);
                     frow_solve(a0, a1, a2, a3, aim, A, B, warm);
                     if (TWO && ch.z > 1) {
                         float4 im = s_p2[4 * TILE_CAP];
@@ -1829,7 +1856,7 @@ B2D_D void island_tiles(const Dev &d, int vel_iters, int pos_iters) {
                         frow_solve(r[0], r[TILE_CAP], r[2 * TILE_CAP], r[3 * TILE_CAP], im, A, B, warm);
                         r[4 * TILE_CAP] = im;
                     }
-                    tf_store(s_body, ch.w & 0xFFFFu, A); tf_store(s_body, ch.w >> 16, B);
+                    tf_store(s_body, slot_a(ch.w), A); tf_store(s_body, slot_b(ch.w), B);
                 }
                 __syncthreads();
             }
@@ -1853,20 +1880,20 @@ B2D_D void island_tiles(const Dev &d, int vel_iters, int pos_iters) {
         a40 = b40 = n40 = l40 = a41 = b41 = n41 = l41 = make_float4(0, 0, 0, 0);
         float4 spos = make_float4(0, 0, 0, 0), sorn = make_float4(0, 0, 0, 1);      // this thread's non-procedural partner (contact, else joint)
         if (hasH) {
-            hisl = d.bslot[island_of(d, hh.x & 0x7FFFFFFFu, hh.y & 0x7FFFFFFFu)];
+            hisl = d.bslot[island_of(d, tag_id(hh.x), tag_id(hh.y))];
             const uint32_t h = hh.z;
             fA0 = mk3(d.hfA0[h]); fB0 = mk3(d.hfB0[h]); pvA = mk3(d.hpivA[h]); pvB = mk3(d.hpivB[h]);
         }
         if (hasC) {
-            cisl = d.bslot[island_of(d, ch.x & 0x7FFFFFFFu, ch.y & 0x7FFFFFFFu)];
+            cisl = d.bslot[island_of(d, tag_id(ch.x), tag_id(ch.y))];
             if (!TWO) {
                 a40 = d.pA[m]; b40 = d.pB[m]; n40 = d.pN[m]; l40 = d.pL[m];
                 if (ch.z > 1) { a41 = d.pA[NM + m]; b41 = d.pB[NM + m]; n41 = d.pN[NM + m]; l41 = d.pL[NM + m]; }
             }
         }
         float4 hpos = spos, horn = sorn;                        // a joint to a static / kinematic body
-        if (hasC && ((ch.x | ch.y) >> 31)) { const uint32_t sbody = ((ch.x >> 31) ? ch.x : ch.y) & 0x7FFFFFFFu; spos = d.pos[sbody]; sorn = d.orn[sbody]; }
-        if (hasH && ((hh.x | hh.y) >> 31)) { const uint32_t sbody = ((hh.x >> 31) ? hh.x : hh.y) & 0x7FFFFFFFu; hpos = d.pos[sbody]; horn = d.orn[sbody]; }
+        if (hasC && ((ch.x | ch.y) >> 31)) { const uint32_t sbody = tag_id(tag_proc(ch.x) ? ch.y : ch.x); spos = d.pos[sbody]; sorn = d.orn[sbody]; }
+        if (hasH && ((hh.x | hh.y) >> 31)) { const uint32_t sbody = tag_id(tag_proc(hh.x) ? hh.y : hh.x); hpos = d.pos[sbody]; horn = d.orn[sbody]; }
         __syncthreads();                                         // the rows in s_row (two-point: s_p2, s_hr) are dead from here on
         if (hasC) for (uint32_t s = TWO ? 0 : 2; s < ch.z; ++s) {
             const size_t mi = s * NM + m;
@@ -1884,22 +1911,21 @@ B2D_D void island_tiles(const Dev &d, int vel_iters, int pos_iters) {
             s_body[5 * TILE_CAP + t] = d.invI[3 * mybody]; s_body[6 * TILE_CAP + t] = d.invI[3 * mybody + 1]; s_body[7 * TILE_CAP + t] = d.invI[3 * mybody + 2];
         }
         __syncthreads();
-        // ---- position iterations: <= N, each island stopping once its max error drops below 0.005 (island_solver.cpp:263-353,
-        // :538-543); per-island error / done words sit at the slot of the island's root body; the contact points of the first two
+        // ---- position iterations: <= N, each island stopping once island_done (island_solver.cpp:263-353); per-island error / done words sit at the slot of the island's root body; the contact points of the first two
         // slots stay in registers, their refreshed normal and distance (contact_constraint.cpp:72-76) are written back at the end
         for (int it = 0; it < pos_iters; ++it) {
             for (uint32_t c = 0; c < nhc; ++c) {
                 if (hcol == c && !s_done[hisl]) {
-                    PBody A, B; tq_load(s_body, hh.x, hh.w & 0xFFFFu, hpos, horn, A); tq_load(s_body, hh.y, hh.w >> 16, hpos, horn, B);
+                    PBody A, B; tq_load(s_body, hh.x, slot_a(hh.w), hpos, horn, A); tq_load(s_body, hh.y, slot_b(hh.w), hpos, horn, B);
                     const float max_error = hinge_position(A, B, fA0, fB0, pvA, pvB);
-                    tq_store(s_body, hh.w & 0xFFFFu, A); tq_store(s_body, hh.w >> 16, B);
+                    tq_store(s_body, slot_a(hh.w), A); tq_store(s_body, slot_b(hh.w), B);
                     tile_error_max(s_err, hisl, max_error);
                 }
                 __syncthreads();
             }
             for (uint32_t c = 0; c < ncc; ++c) {
                 if (ccol == c && !s_done[cisl]) {
-                    PBody A, B; tq_load(s_body, ch.x, ch.w & 0xFFFFu, spos, sorn, A); tq_load(s_body, ch.y, ch.w >> 16, spos, sorn, B);
+                    PBody A, B; tq_load(s_body, ch.x, slot_a(ch.w), spos, sorn, A); tq_load(s_body, ch.y, slot_b(ch.w), spos, sorn, B);
                     float max_error = 0.0f;
                     if (!TWO) {
                         contact_point_position(A, B, a40, b40, n40, l40, max_error);
@@ -1911,13 +1937,13 @@ B2D_D void island_tiles(const Dev &d, int vel_iters, int pos_iters) {
                         contact_point_position(A, B, pa, r[TILE_CAP], pn, r[3 * TILE_CAP], max_error);
                         r[0] = pa; r[2 * TILE_CAP] = pn;
                     }
-                    tq_store(s_body, ch.w & 0xFFFFu, A); tq_store(s_body, ch.w >> 16, B);
+                    tq_store(s_body, slot_a(ch.w), A); tq_store(s_body, slot_b(ch.w), B);
                     tile_error_max(s_err, cisl, max_error);
                 }
                 __syncthreads();
             }
             if (it + 1 < pos_iters) {
-                if (t < nb && s_root[t]) { if (__uint_as_float(s_err[t]) < 0.005f) s_done[t] = 1; s_err[t] = 0; }
+                if (t < nb && s_root[t]) { if (island_done(__uint_as_float(s_err[t]))) s_done[t] = 1; s_err[t] = 0; }
                 __syncthreads();
             }
         }
@@ -1949,13 +1975,6 @@ __global__ void __launch_bounds__(TILE_CAP, 2) k_island_tiles_2p(Dev d, int vel_
 #ifndef B2D_POS_THREADS
 #define B2D_POS_THREADS 256
 #endif
-struct PTicket { uint32_t ta, tb, mask; bool on; };
-B2D_D PTicket pticket_of(uint2 tk, int it, uint32_t mask, bool on) {
-    PTicket t; t.on = on; t.mask = mask;
-    const uint32_t SA = (tk.x & 0xFFu) - ((tk.x >> 16) & 0xFFu), SB = (tk.y & 0xFFu) - ((tk.y >> 16) & 0xFFu);
-    t.ta = (uint32_t)it * SA + ((tk.x >> 8) & 0xFFu); t.tb = (uint32_t)it * SB + ((tk.y >> 8) & 0xFFu);
-    return t;
-}
 
 // ---- dataflow flavour of the position iterations (default).  Same idea as k_solve_df: what a constraint needs from a
 // body AND the body's ticket travel in the same 16-byte vectors, so a poll that sees the expected ticket in all three
@@ -1997,15 +2016,17 @@ B2D_D void pb_begin(const Dev &d, uint32_t id, bool proc, PBody &b, m3 &stale) {
 // One chunk of position constraints.  `work` runs the constraint on (A, B) and returns its max error.
 template<typename Work>
 B2D_D void position_chunk_df(const Dev &d, uint32_t tagA, uint32_t tagB, uint2 tk2, uint32_t isl, int it, uint32_t mask, Work work) {
-    const uint32_t a = tagA & 0x7FFFFFFFu, b = tagB & 0x7FFFFFFFu;
-    const bool pa = !(tagA >> 31), pb = !(tagB >> 31);
+    const uint32_t a = tag_id(tagA), b = tag_id(tagB);
+    const bool pa = tag_proc(tagA), pb = tag_proc(tagB);
     // all constraints of a finished island skip together (and keep skipping), so their tickets stay consistent
     const bool skip = __ldcg(&d.isl_done[isl]) != 0;
     PBody A, B; m3 staleA, staleB;
     pb_begin(d, a, pa, A, staleA); pb_begin(d, b, pb, B, staleB);
     const uint32_t live = __ballot_sync(mask, !skip);
     if (skip) return;
-    const PTicket tk = pticket_of(tk2, it, live, true);
+    const Ticket tk = ticket_of(tk2, it, PASS_POSITION, live);
+    // ticket_wait's loop, written out: through the template k_position_df needs 2 more registers (ptxas, sm_90a).  Unlike
+    // ticket_wait it polls whether or not the lane is pending; a lane that is done finds its bodies past its tickets.
     bool pending = true; uint32_t spins = 0;
     do {
         PRec ra, rb;
@@ -2021,11 +2042,7 @@ B2D_D void position_chunk_df(const Dev &d, uint32_t tagA, uint32_t tagB, uint2 t
             island_error_max(d, isl, max_error);
             pending = false;
         }
-        if (!__any_sync(live, pending)) break;
-        if (!__any_sync(live, ok)) {
-            if (++spins > (1u << 20)) { atomicOr(&d.cnt->err, ERR_SOLVER_TIMEOUT); break; }      // never hang the GPU
-            if (spins > 64) __nanosleep(20);
-        }
+        if (!acquire_more(d, tk, pending, ok, spins)) break;
     } while (true);
 }
 // contact_constraint::solve_position, contact_constraint.cpp:58-90
@@ -2050,20 +2067,16 @@ B2D_D void hinge_position_df(const Dev &d, uint4 hd, uint2 tk2, uint32_t isl, in
     const v3 fA0 = mk3(d.hfA0[h]), fB0 = mk3(d.hfB0[h]), pvA = mk3(d.hpivA[h]), pvB = mk3(d.hpivB[h]);
     position_chunk_df(d, hd.x, hd.y, tk2, isl, it, mask, [&](PBody &A, PBody &B) { return hinge_position(A, B, fA0, fB0, pvA, pvB); });
 }
+// what the position iterations fetch one chunk ahead: also the island label and the manifold slot
+struct PositionHead {
+    uint4 hd; uint2 tk; uint32_t isl, m;
+    B2D_D void fetch(const Dev &d, uint32_t i) { hd = d.hdr[i]; tk = d.tkt[i]; isl = d.pisl[i]; m = d.cidx_s[i]; }
+};
 __global__ void __launch_bounds__(B2D_POS_THREADS, B2D_POS_MIN_BLOCKS) k_position_df(Dev d, int iters) {
-    __shared__ uint32_t s_coff[MAX_COLORS + 2], s_cchunk[MAX_COLORS + 2], s_hoff[MAX_COLORS + 2], s_hchunk[MAX_COLORS + 2];
+    __shared__ ChunkTables tables;
     GridBarrier grid(&d.cnt->bar);
-    const Counters &c = *d.cnt;
-    if (threadIdx.x < MAX_COLORS + 2) {
-        s_coff[threadIdx.x] = c.coff[threadIdx.x]; s_cchunk[threadIdx.x] = c.cchunk[threadIdx.x];
-        s_hoff[threadIdx.x] = c.hoff[threadIdx.x]; s_hchunk[threadIdx.x] = c.hchunk[threadIdx.x];
-    }
-    const uint32_t nc = c.ncolors, nh = c.nhcolors;
-    __syncthreads();
-    const uint32_t lane = threadIdx.x & 31u;
-    const uint32_t wid = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
-    const uint32_t hchunks = s_hchunk[nh], cchunks = s_cchunk[nc];
-    if (hchunks + cchunks == 0) return;               // every island is tiled (the whole grid takes this exit together)
+    ChunkWalk<PositionHead> walk(d, tables);
+    if (walk.hchunks + walk.cchunks == 0) return;       // every island is tiled (the whole grid takes this exit together)
     GRID_STRIDE(i, d.nbodies) {
         d.isl_err[i] = 0; d.isl_done[i] = 0;
         if (is_dynamic(d.flags[i])) {
@@ -2072,34 +2085,17 @@ __global__ void __launch_bounds__(B2D_POS_THREADS, B2D_POS_MIN_BLOCKS) k_positio
             r[0] = make_float4(p4.x, p4.y, p4.z, 0.0f); r[1] = make_float4(o4.x, o4.y, o4.z, 0.0f); r[2] = make_float4(o4.w, 0.0f, 0.0f, 0.0f);
         }
     }
-    // header, ticket and island words of this warp's next contact chunk are fetched one chunk ahead (as in k_solve_df)
-    uint32_t ncol = 0, ni = 0, nisl = 0, nm = 0; bool nact = false; uint4 nhd = make_uint4(0, 0, 0, 0); uint2 ntk = make_uint2(0, 0);
-    if (wid < cchunks) {
-        ni = chunk_index(s_cchunk, s_coff, wid, ncol) + lane; nact = ni < s_coff[ncol + 1];
-        if (nact) { nhd = d.hdr[ni]; ntk = d.tkt[ni]; nisl = d.pisl[ni]; nm = d.cidx_s[ni]; }
-    }
+    walk.start(d);
     grid.sync();
     for (int it = 0; it < iters; ++it) {
-        { uint32_t col = 0;
-          for (uint32_t j = wid; j < hchunks; j += nw) {
-              const uint32_t i = chunk_index(s_hchunk, s_hoff, j, col) + lane;
-              const bool act = i < s_hoff[col + 1];
-              const uint32_t mask = __ballot_sync(0xffffffffu, act);
-              if (act) hinge_position_df(d, d.hhdr[i], d.htkt[i], d.hisl[i], it, mask);
-          } }
-        for (uint32_t j = wid; j < cchunks; j += nw) {
-            const bool act = nact; const uint4 hd = nhd; const uint2 tk2 = ntk; const uint32_t isl = nisl, m = nm;
-            uint32_t jn = j + nw;
-            if (jn >= cchunks) { jn = wid; ncol = 0; }
-            ni = chunk_index(s_cchunk, s_coff, jn, ncol) + lane; nact = ni < s_coff[ncol + 1];
-            if (nact) { nhd = d.hdr[ni]; ntk = d.tkt[ni]; nisl = d.pisl[ni]; nm = d.cidx_s[ni]; }
-            const uint32_t mask = __ballot_sync(0xffffffffu, act);
-            if (act) contact_position_df(d, hd, m, tk2, isl, it, mask);
-        }
+        walk.hinges([&](uint32_t i, uint32_t mask) { hinge_position_df(d, d.hhdr[i], d.htkt[i], d.hisl[i], it, mask); });
+        walk.contacts(d, [](uint32_t, bool) {}, [&](uint32_t, const PositionHead &h, uint32_t mask) {
+            contact_position_df(d, h.hd, h.m, h.tk, h.isl, it, mask);
+        });
         if (it + 1 < iters) {
             grid.sync();
             GRID_STRIDE(i, d.nbodies) {
-                if (d.parent[i] == i) { if (__uint_as_float(d.isl_err[i]) < 0.005f) d.isl_done[i] = 1; d.isl_err[i] = 0; }
+                if (d.parent[i] == i) { if (island_done(__uint_as_float(d.isl_err[i]))) d.isl_done[i] = 1; d.isl_err[i] = 0; }
             }
             grid.sync();
         }
@@ -2261,22 +2257,7 @@ B2D_D void rest_solve_group(const Dev &d, const uint32_t *group, int ng) {
         const q4 ornA = mkq(d.orn[pr.x]), ornB = mkq(d.orn[pr.y]);
         for (uint32_t s = 0; s < npts; ++s) {
             if (nr == REST_MAX_ROWS) { atomicOr(&d.cnt->err, ERR_RESTITUTION_GROUP); break; }
-            const size_t mi = (size_t)s * d.NM + m;
-            const float4 a4 = d.pA[mi], b4 = d.pB[mi], n4 = d.pN[mi];
-            const v3 normal = mk3(n4);
-            const v3 pAw = to_world(mk3(a4), posA, ornA), pBw = to_world(mk3(b4), posB, ornB);
-            const v3 rA = pAw - posA, rB = pBw - posB;
-            const v3 J1 = cross(rA, normal), J2 = -normal, J3 = -cross(rB, normal);
-            const float em = eff_mass(normal, J1, J2, J3, A, B);
-            const float relvel = rel_speed(normal, J1, J2, J3, A.v, A.w, B.v, B.w);
-            const float rhs = -(0.0f * 0.2f + relvel * (1.0f + n4.w));              // constraint_row_options{}: error 0, the point's restitution
-            v3 t, u; plane_space(normal, t, u);
-            const v3 T1 = cross(rA, t), T2 = -t, T3 = -cross(rB, t);
-            const v3 U1 = cross(rA, u), U2 = -u, U3 = -cross(rB, u);
-            r0[nr] = f4(normal, rhs); r1[nr] = f4(rA, em); r2[nr] = f4(rB, b4.w);
-            r3[nr] = make_float4(eff_mass(t, T1, T2, T3, A, B), eff_mass(u, U1, U2, U3, A, B),
-                                 -rel_speed(t, T1, T2, T3, A.v, A.w, B.v, B.w), -rel_speed(u, U1, U2, U3, A.v, A.w, B.v, B.w));
-            im[nr] = make_float4(0, 0, 0, 0);
+            contact_point_rows(d, (size_t)s * d.NM + m, A, B, posA, ornA, posB, ornB, r0[nr], r1[nr], r2[nr], r3[nr], im[nr], true);
             ra[nr] = pr.x; rb[nr] = pr.y;
             ++nr;
         }

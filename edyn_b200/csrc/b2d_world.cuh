@@ -172,7 +172,7 @@ struct Dev {
     double *isl_ts, *ts_new;
     uint32_t *pisl, *hisl;       // per sorted constraint: island label (position solver early exit)
     float4 *prec;                // position solver: 3 float4 per body, (pos,t) (orn.xyz,t) (orn.w,fresh,0,t)
-    uint2 *tkt, *htkt;           // per sorted constraint, per body side: S | base << 8 | k << 16 (see k_prepare_*)
+    uint2 *tkt, *htkt;           // per sorted constraint, per body side: S | base << 8 | k << 16 (see ticket_word)
 
     // ---- multi-GPU hand-over (b2d_dist.cuh): scene-global body names and the island / destination scratch
     uint32_t *entity;                    // scene-global name per body (entt::entity in the EnTT binding); default = local id
