@@ -123,12 +123,6 @@ static cudaError_t coop_launch(b2d_world *w, K kernel, int blocks, int threads, 
     return cudaLaunchCooperativeKernel((void *)kernel, dim3(blocks), dim3(threads), params, 0, w->stream);
 }
 
-template<int FN> static void launch_detect(b2d_world *w) {
-    Dev &d = w->d;
-    // heavy overloads (box-box, capsule-box) get a full grid; the others are short
-    LAUNCH(k_np_detect<FN>, d.NM, 128, d);
-}
-
 extern "C" {
 
 const char *b2d_last_error(const b2d_world *w) { return w ? w->error.c_str() : g_create_error.c_str(); }
@@ -172,7 +166,7 @@ b2d_world *b2d_create(const b2d_config *cfg) {
     d.xhash_size = 0; d.xhash_key = nullptr;
     ok = ok && dalloc(w, d.mpair, NM) && dalloc(w, d.mstate, NM);
     ok = ok && dalloc(w, d.pA, 4 * (size_t)NM) && dalloc(w, d.pB, 4 * (size_t)NM) && dalloc(w, d.pN, 4 * (size_t)NM);
-    ok = ok && dalloc(w, d.pL, 4 * (size_t)NM) && dalloc(w, d.pI, 4 * (size_t)NM) && dalloc(w, d.npres, NM) && dalloc(w, d.clist, NM);
+    ok = ok && dalloc(w, d.pL, 4 * (size_t)NM) && dalloc(w, d.pI, 4 * (size_t)NM) && dalloc(w, d.clist, NM);
     ok = ok && dalloc(w, d.parent, NB) && dalloc(w, d.bmask, NB) && dalloc(w, d.jmask, NB) && dalloc(w, d.prop, NB) && dalloc(w, d.jprop, NB);
     ok = ok && dalloc(w, d.ckey, NM) && dalloc(w, d.ckey_s, NM) && dalloc(w, d.cidx, NM) && dalloc(w, d.cidx_s, NM) && dalloc(w, d.npidx, NM);
     ok = ok && dalloc(w, d.hkey, NH) && dalloc(w, d.hkey_s, NH) && dalloc(w, d.hidx, NH) && dalloc(w, d.hidx_s, NH);
@@ -577,9 +571,9 @@ static int enqueue_narrowphase(b2d_world *w) {
     CK(cudaMemsetAsync(d.cnt->npcount, 0, 32 * sizeof(uint32_t), s));        // histogram + cursors
     LAUNCH(k_np_keys, d.NM, 256, d);
     LAUNCH(k_np_scatter, d.NM, 256, d);           // CTAs of exactly 256 threads (window size)
-    LAUNCH(k_np_detect_light, d.NM, 128, d);
-    launch_detect<5>(w); launch_detect<9>(w);
-    LAUNCH(k_np_merge, d.NM, 128, d);
+    LAUNCH(k_np_collide_light, d.NM, 128, d);
+    LAUNCH(k_np_collide<5>, d.NM, 128, d);
+    LAUNCH(k_np_collide<9>, d.NM, 128, d);
     return B2D_OK;
 }
 // connected components over the current edges (manifolds + joints): island label per body

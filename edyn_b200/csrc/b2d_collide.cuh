@@ -785,18 +785,24 @@ B2D_D int pair_fn(int a, int b) {
     if (a == SH_CAPSULE && b == SH_BOX) return 9;
     return 0;
 }
-B2D_D void run_pair(int fn, float4 A, float4 B, const CCtx &c, CResult &r) {
+// the seven light overloads; box-box (5) and capsule-box (9) are not called from here
+B2D_D void run_light_pair(int fn, float4 A, float4 B, const CCtx &c, CResult &r) {
     switch (fn) {
     case 1: collide_sphere_sphere(A, B, c, r); break;
     case 2: collide_sphere_plane(A, B, c, r); break;
     case 3: collide_sphere_box(A, B, c, r); break;
     case 4: collide_box_plane(A, B, c, r); break;
-    case 5: collide_box_box(A, B, c, r); break;
     case 6: collide_capsule_plane(A, B, c, r); break;
     case 7: collide_capsule_capsule(A, B, c, r); break;
     case 8: collide_capsule_sphere(A, B, c, r); break;
-    case 9: collide_capsule_box(A, B, c, r); break;
     default: break;
+    }
+}
+B2D_D void run_pair(int fn, float4 A, float4 B, const CCtx &c, CResult &r) {
+    switch (fn) {
+    case 5: collide_box_box(A, B, c, r); break;
+    case 9: collide_capsule_box(A, B, c, r); break;
+    default: run_light_pair(fn, A, B, c, r); break;
     }
 }
 B2D_D void collide(int kindA, float4 A, int kindB, float4 B, const CCtx &c, CResult &r) {

@@ -463,13 +463,12 @@ B2D_D MPoint create_point(const CPoint &rp, q4 ornA, q4 ornB, float2 matA, float
     return cp;
 }
 
-// Narrowphase in three kernels:
+// Narrowphase in three steps:
 //   k_np_keys     pair-type key per manifold slot + histogram, k_np_scatter the counting sort by type, so that
-//   k_np_detect<FN> runs ONE collide() overload per launch over a contiguous range of the sorted list
-//                 (no intra-warp divergence between sphere/box/capsule code paths); the <= 4 result points go to
-//                 the solver-row arrays R0/R1/R2, which are idle in this phase;
-//   k_np_merge    update_contact_distances (collision_util.cpp:28-45) + process_collision
-//                 (collision_util.hpp:105-276, sequential flavour of narrowphase.hpp:62-84) per manifold.
+//   k_np_collide  runs the collision of every awake manifold over the sorted list, where a warp's lanes run the same
+//                 collide() overload (no divergence between sphere/box/capsule code paths but at the range edges),
+//                 and merges the result, still in registers, into the manifold's points (np_merge).
+//                 k_np_collide<5> (box-box) and <9> (capsule-box) take a launch each, k_np_collide_light the rest.
 __global__ void k_np_keys(Dev d) {
     __shared__ uint32_t s_hist[16];
     if (threadIdx.x < 16) s_hist[threadIdx.x] = 0;
@@ -525,144 +524,138 @@ __global__ void __launch_bounds__(256) k_np_scatter(Dev d) {
     }
 }
 
-template<int FN>
-B2D_D void np_detect_range(const Dev &d) {
+// update_contact_distances (collision_util.cpp:28-45) + process_collision (collision_util.hpp:105-276, sequential flavour
+// of narrowphase.hpp:62-84) of alive, awake manifold m in state st between bodies pr.x (flags fa, pose posA ornA) and
+// pr.y, with this step's collision result res
+B2D_D void np_merge(const Dev &d, uint32_t m, uint32_t st, uint2 pr, uint32_t fa, uint32_t fb,
+                    v3 posA, q4 ornA, v3 posB, q4 ornB, const CResult &res) {
+    int num = (int)(st & MS_NPTS_MASK);
+    if (num == 0 && res.num == 0) return;
+    const uint32_t a = pr.x, b = pr.y;
+    MPoint P[4];
+    for (int s = 0; s < num; ++s) {
+        load_point(d, m, s, P[s]);
+        v3 pAw = to_world(P[s].pivotA, posA, ornA), pBw = to_world(P[s].pivotB, posB, ornB);
+        P[s].distance = dot(P[s].normal, pAw - pBw);
+    }
+    // ---- merge with persisted points
+    bool merged[4] = {false, false, false, false};
+    const bool rollA = fa & F_ROLLING, rollB = fb & F_ROLLING;
+    int i = 0;
+    while (i < num) {
+        MPoint &cp = P[i];
+        ++cp.lifetime;
+        int nearest = find_nearest_contact(cp.pivotA, cp.pivotB, res);
+        if (nearest == res.num && rollA) nearest = find_nearest_contact_rolling(res, cp.pivotA, posA, ornA, mk3(d.angvel[a]), d.dt);
+        if (nearest == res.num && rollB) nearest = find_nearest_contact_rolling(res, cp.pivotB, posB, ornB, mk3(d.angvel[b]), d.dt);
+        bool remove = false;
+        if (nearest < res.num && !merged[nearest]) { merge_point(res.pt[nearest], cp, ornA, ornB); merged[nearest] = true; }
+        else {                                          // should_remove_point, collision_util.cpp:397-413
+            v3 pA = to_world(cp.pivotA, posA, ornA), pB = to_world(cp.pivotB, posB, ornB);
+            v3 dd = pA - pB;
+            float nd = dot(dd, cp.normal);
+            v3 td = dd - nd * cp.normal;
+            remove = nd > BREAKING_THRESHOLD || length_sqr(td) > BREAKING_THRESHOLD * BREAKING_THRESHOLD;
+        }
+        if (remove) { for (int k = i + 1; k < num; ++k) P[k - 1] = P[k]; --num; }
+        else ++i;
+    }
+    bool all = true;
+    for (int k = 0; k < res.num; ++k) all = all && merged[k];
+    if (!all) {
+        CPoint L[4]; int ent[4] = {-1, -1, -1, -1}; int type[4] = {INS_NONE, INS_NONE, INS_NONE, INS_NONE};
+        int num_points = num;
+        if (num_points > 0) {
+            for (int k = 0; k < num; ++k) { L[k].pivotA = P[k].pivotA; L[k].pivotB = P[k].pivotB; L[k].normal = P[k].normal; L[k].distance = P[k].distance; L[k].att = ATT_NONE; ent[k] = k; }
+        } else {
+            num_points = 1; L[0] = res.pt[0]; type[0] = INS_APPEND; merged[0] = true;
+        }
+        for (int k = 0; k < res.num; ++k) {
+            if (merged[k]) continue;
+            v3 piv[4];
+            for (int j = 0; j < num_points; ++j) piv[j] = L[j].pivotA;
+            int idx;
+            int t = insertion_point_index(piv, num_points, res.pt[k].pivotA, idx);
+            if (t == INS_NONE) {
+                for (int j = 0; j < num_points; ++j) piv[j] = L[j].pivotB;
+                t = insertion_point_index(piv, num_points, res.pt[k].pivotB, idx);
+            }
+            if (t != INS_NONE && idx >= 0 && idx < 4) { L[idx] = res.pt[k]; type[idx] = t; }
+        }
+        const float2 matA = d.mat[a], matB = d.mat[b];
+        MPoint created[4]; int n_created = 0;
+        bool alive[4] = {true, true, true, true};
+        for (int k = 0; k < num_points; ++k) {
+            if (type[k] == INS_APPEND) created[n_created++] = create_point(L[k], ornA, ornB, matA, matB);
+            else if (type[k] == INS_SIMILAR) {
+                if (ent[k] < 0) created[n_created++] = create_point(L[k], ornA, ornB, matA, matB);
+                else merge_point(L[k], P[ent[k]], ornA, ornB);
+            } else if (type[k] == INS_REPLACE) {
+                if (ent[k] >= 0) alive[ent[k]] = false;
+                created[n_created++] = create_point(L[k], ornA, ornB, matA, matB);
+            }
+        }
+        MPoint Q[4]; int w = 0;
+        for (int k = n_created - 1; k >= 0; --k) Q[w++] = created[k];      // newest point = list head
+        for (int k = 0; k < num; ++k) if (alive[k] && w < 4) Q[w++] = P[k];
+        num = w;
+        for (int k = 0; k < num; ++k) P[k] = Q[k];
+    }
+    for (int s = 0; s < num; ++s) store_point(d, m, s, P[s]);
+    d.mstate[m] = (st & ~MS_NPTS_MASK) | (uint32_t)num;
+    // the island rebuild reads whether a manifold has points (colouring, island census) and, on the dataflow path,
+    // its point count (sort key); inside an island tile the count only matters to the solver itself, except that a
+    // two-point tile has no room for a third point
+    const uint32_t was = st & MS_NPTS_MASK;
+    if ((uint32_t)num != was) {
+        const uint32_t tile = d.btile[key_body(d, pr)];
+        if (was == 0u || num == 0 || tile == TILE_NONE || (num > 2 && was <= 2u && tile < d.cnt->ntiles2)) d.cnt->graph_changed = 1u;
+    }
+}
+// detect_collision (collision_util.cpp:440-475) of the manifold at position i of the sorted list, then its np_merge.
+// FN is the ordered pair type of the launch, 0 in the light launch, which takes it from the shapes at run time.  Sleeping
+// manifolds are not in the list: their points and lifetimes stay untouched.
+template <int FN>
+B2D_D void np_run(int fn, float4 A, float4 B, const CCtx &c, CResult &r) {
+    if constexpr (FN != 0) run_pair(FN, A, B, c, r); else run_light_pair(fn, A, B, c, r);
+}
+template <int FN>
+B2D_D void np_manifold(const Dev &d, uint32_t i) {
+    const uint32_t m = d.npidx[i];
+    const uint32_t st = d.mstate[m];
+    const uint2 pr = d.mpair[m];
+    const uint32_t fa = d.flags[pr.x], fb = d.flags[pr.y];
+    // the AABB gate, collision_util.cpp:444-474; a manifold it closes still merges an empty result into its points
+    const bool near = intersect(inset(body_box(d, pr.x), -BREAKING_THRESHOLD), body_box(d, pr.y));
+    if (!near && !(st & MS_NPTS_MASK)) return;
+    const v3 posA = mk3(d.pos[pr.x]), posB = mk3(d.pos[pr.y]);
+    const q4 ornA = mkq(d.orn[pr.x]), ornB = mkq(d.orn[pr.y]);
+    CResult res; res.num = 0;
+    if (near) {
+        const int ka = shape_of(fa), kb = shape_of(fb);
+        const int fn = pair_fn(ka, kb);             // the list holds type FN = pair_fn(ka, kb), or pair_fn(kb, ka) if that is 0
+        CCtx ctx; ctx.threshold = COLLISION_THRESHOLD;
+        if (fn) {
+            ctx.posA = posA; ctx.ornA = ornA; ctx.posB = posB; ctx.ornB = ornB;
+            np_run<FN>(fn, d.shp[pr.x], d.shp[pr.y], ctx, res);
+        } else {                                    // swap_collide, collide.hpp:369-374
+            ctx.posA = posB; ctx.ornA = ornB; ctx.posB = posA; ctx.ornB = ornA;
+            np_run<FN>(pair_fn(kb, ka), d.shp[pr.y], d.shp[pr.x], ctx, res);
+            swap_result(res);
+        }
+    }
+    np_merge(d, m, st, pr, fa, fb, posA, ornA, posB, ornB, res);
+}
+// the two heavy overloads (box-box, capsule-box) get a launch each over their range of the list
+template <int FN>
+__global__ void __launch_bounds__(128) k_np_collide(Dev d) {
     const uint32_t b = d.cnt->npoff[FN], e = d.cnt->npoff[FN + 1];
-    for (uint32_t i = b + blockIdx.x * blockDim.x + threadIdx.x; i < e; i += gridDim.x * blockDim.x) {
-        const uint32_t m = d.npidx[i];
-        const uint2 pr = d.mpair[m];
-        const uint32_t fa = d.flags[pr.x], fb = d.flags[pr.y];
-        CResult res; res.num = 0;
-        // detect_collision's AABB gate, collision_util.cpp:444-474
-        if (intersect(inset(body_box(d, pr.x), -BREAKING_THRESHOLD), body_box(d, pr.y))) {
-            const int ka = shape_of(fa), kb = shape_of(fb);
-            CCtx ctx; ctx.threshold = COLLISION_THRESHOLD;
-            if (pair_fn(ka, kb) == FN) {
-                ctx.posA = mk3(d.pos[pr.x]); ctx.ornA = mkq(d.orn[pr.x]); ctx.posB = mk3(d.pos[pr.y]); ctx.ornB = mkq(d.orn[pr.y]);
-                run_pair(FN, d.shp[pr.x], d.shp[pr.y], ctx, res);
-            } else {                                    // swap_collide, collide.hpp:369-374
-                ctx.posA = mk3(d.pos[pr.y]); ctx.ornA = mkq(d.orn[pr.y]); ctx.posB = mk3(d.pos[pr.x]); ctx.ornB = mkq(d.orn[pr.x]);
-                run_pair(FN, d.shp[pr.y], d.shp[pr.x], ctx, res);
-                swap_result(res);
-            }
-        }
-        d.npres[m] = (unsigned char)res.num;
-        for (int s = 0; s < res.num; ++s) {
-            size_t ri = (size_t)s * d.NM + m;
-            d.R0[ri] = f4(res.pt[s].pivotA, res.pt[s].distance);
-            d.R1[ri] = f4(res.pt[s].pivotB, __uint_as_float(res.pt[s].att));
-            d.R2[ri] = f4(res.pt[s].normal, 0);
-        }
-    }
+    for (uint32_t i = b + blockIdx.x * blockDim.x + threadIdx.x; i < e; i += gridDim.x * blockDim.x) np_manifold<FN>(d, i);
 }
-// the two heavy overloads (box-box, capsule-box) get a launch each, the seven light ones share one
-template<int FN>
-__global__ void __launch_bounds__(128) k_np_detect(Dev d) { np_detect_range<FN>(d); }
-__global__ void __launch_bounds__(128) k_np_detect_light(Dev d) {
-    np_detect_range<1>(d); np_detect_range<2>(d); np_detect_range<3>(d); np_detect_range<4>(d);
-    np_detect_range<6>(d); np_detect_range<7>(d); np_detect_range<8>(d);
-}
-
-__global__ void __launch_bounds__(128) k_np_merge(Dev d) {
-    const uint32_t hwm = d.cnt->hwm;
-    GRID_STRIDE(m, hwm) {
-        uint32_t st = d.mstate[m];
-        if (!(st & MS_ALIVE)) continue;
-        int num = (int)(st & MS_NPTS_MASK);
-        CResult res; res.num = d.npres[m];
-        if (num == 0 && res.num == 0) continue;
-        uint2 pr = d.mpair[m];
-        const uint32_t a = pr.x, b = pr.y;
-        const uint32_t fa = d.flags[a], fb = d.flags[b];
-        if (!is_dynamic(fa) && !is_dynamic(fb)) continue;          // sleeping manifold (npres is stale): points, lifetimes untouched
-        const v3 posA = mk3(d.pos[a]), posB = mk3(d.pos[b]);
-        const q4 ornA = mkq(d.orn[a]), ornB = mkq(d.orn[b]);
-        for (int s = 0; s < res.num; ++s) {
-            size_t ri = (size_t)s * d.NM + m;
-            float4 r0 = d.R0[ri], r1 = d.R1[ri], r2 = d.R2[ri];
-            res.pt[s].pivotA = mk3(r0); res.pt[s].distance = r0.w; res.pt[s].pivotB = mk3(r1); res.pt[s].att = __float_as_uint(r1.w);
-            res.pt[s].normal = mk3(r2);
-        }
-        MPoint P[4];
-        for (int s = 0; s < num; ++s) {
-            load_point(d, m, s, P[s]);
-            v3 pAw = to_world(P[s].pivotA, posA, ornA), pBw = to_world(P[s].pivotB, posB, ornB);
-            P[s].distance = dot(P[s].normal, pAw - pBw);
-        }
-        // ---- merge with persisted points
-        bool merged[4] = {false, false, false, false};
-        const bool rollA = fa & F_ROLLING, rollB = fb & F_ROLLING;
-        int i = 0;
-        while (i < num) {
-            MPoint &cp = P[i];
-            ++cp.lifetime;
-            int nearest = find_nearest_contact(cp.pivotA, cp.pivotB, res);
-            if (nearest == res.num && rollA) nearest = find_nearest_contact_rolling(res, cp.pivotA, posA, ornA, mk3(d.angvel[a]), d.dt);
-            if (nearest == res.num && rollB) nearest = find_nearest_contact_rolling(res, cp.pivotB, posB, ornB, mk3(d.angvel[b]), d.dt);
-            bool remove = false;
-            if (nearest < res.num && !merged[nearest]) { merge_point(res.pt[nearest], cp, ornA, ornB); merged[nearest] = true; }
-            else {                                          // should_remove_point, collision_util.cpp:397-413
-                v3 pA = to_world(cp.pivotA, posA, ornA), pB = to_world(cp.pivotB, posB, ornB);
-                v3 dd = pA - pB;
-                float nd = dot(dd, cp.normal);
-                v3 td = dd - nd * cp.normal;
-                remove = nd > BREAKING_THRESHOLD || length_sqr(td) > BREAKING_THRESHOLD * BREAKING_THRESHOLD;
-            }
-            if (remove) { for (int k = i + 1; k < num; ++k) P[k - 1] = P[k]; --num; }
-            else ++i;
-        }
-        bool all = true;
-        for (int k = 0; k < res.num; ++k) all = all && merged[k];
-        if (!all) {
-            CPoint L[4]; int ent[4] = {-1, -1, -1, -1}; int type[4] = {INS_NONE, INS_NONE, INS_NONE, INS_NONE};
-            int num_points = num;
-            if (num_points > 0) {
-                for (int k = 0; k < num; ++k) { L[k].pivotA = P[k].pivotA; L[k].pivotB = P[k].pivotB; L[k].normal = P[k].normal; L[k].distance = P[k].distance; L[k].att = ATT_NONE; ent[k] = k; }
-            } else {
-                num_points = 1; L[0] = res.pt[0]; type[0] = INS_APPEND; merged[0] = true;
-            }
-            for (int k = 0; k < res.num; ++k) {
-                if (merged[k]) continue;
-                v3 piv[4];
-                for (int j = 0; j < num_points; ++j) piv[j] = L[j].pivotA;
-                int idx;
-                int t = insertion_point_index(piv, num_points, res.pt[k].pivotA, idx);
-                if (t == INS_NONE) {
-                    for (int j = 0; j < num_points; ++j) piv[j] = L[j].pivotB;
-                    t = insertion_point_index(piv, num_points, res.pt[k].pivotB, idx);
-                }
-                if (t != INS_NONE && idx >= 0 && idx < 4) { L[idx] = res.pt[k]; type[idx] = t; }
-            }
-            const float2 matA = d.mat[a], matB = d.mat[b];
-            MPoint created[4]; int n_created = 0;
-            bool alive[4] = {true, true, true, true};
-            for (int k = 0; k < num_points; ++k) {
-                if (type[k] == INS_APPEND) created[n_created++] = create_point(L[k], ornA, ornB, matA, matB);
-                else if (type[k] == INS_SIMILAR) {
-                    if (ent[k] < 0) created[n_created++] = create_point(L[k], ornA, ornB, matA, matB);
-                    else merge_point(L[k], P[ent[k]], ornA, ornB);
-                } else if (type[k] == INS_REPLACE) {
-                    if (ent[k] >= 0) alive[ent[k]] = false;
-                    created[n_created++] = create_point(L[k], ornA, ornB, matA, matB);
-                }
-            }
-            MPoint Q[4]; int w = 0;
-            for (int k = n_created - 1; k >= 0; --k) Q[w++] = created[k];      // newest point = list head
-            for (int k = 0; k < num; ++k) if (alive[k] && w < 4) Q[w++] = P[k];
-            num = w;
-            for (int k = 0; k < num; ++k) P[k] = Q[k];
-        }
-        for (int s = 0; s < num; ++s) store_point(d, m, s, P[s]);
-        d.mstate[m] = (st & ~MS_NPTS_MASK) | (uint32_t)num;
-        // the island rebuild reads whether a manifold has points (colouring, island census) and, on the dataflow path,
-        // its point count (sort key); inside an island tile the count only matters to the solver itself, except that a
-        // two-point tile has no room for a third point
-        const uint32_t was = st & MS_NPTS_MASK;
-        if ((uint32_t)num != was) {
-            const uint32_t tile = d.btile[key_body(d, pr)];
-            if (was == 0u || num == 0 || tile == TILE_NONE || (num > 2 && was <= 2u && tile < d.cnt->ntiles2)) d.cnt->graph_changed = 1u;
-        }
-    }
+// the seven light ones share one: types 1-4 and 6-8, two ranges of the list walked as one
+__global__ void __launch_bounds__(128) k_np_collide_light(Dev d) {
+    const uint32_t b0 = d.cnt->npoff[1], n0 = d.cnt->npoff[5] - b0, b1 = d.cnt->npoff[6], n = n0 + d.cnt->npoff[9] - b1;
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) np_manifold<0>(d, j < n0 ? b0 + j : b1 + (j - n0));
 }
 
 // ====================================================================== islands (connected components)
@@ -1569,39 +1562,38 @@ B2D_D void integrate_body(v3 &v, v3 &w, v3 &pos, q4 &orn, v3 dv, v3 dw, float dt
 }
 // update_aabbs + update_inertias (solver.cpp:453-465) of body i at (pos, orn): the AABB of a shaped body, the world-space
 // inverse inertia of a dynamic one
-B2D_D void refresh_body(const Dev &d, uint32_t i, uint32_t f, v3 pos, q4 orn, float inv_m) {
+B2D_D void refresh_aabb(const Dev &d, uint32_t i, uint32_t f, v3 pos, q4 orn) {
     const int sk = shape_of(f);
     if (sk != SH_NONE) { box3 bb = shape_aabb(sk, d.shp[i], pos, orn); d.bbmin[i] = f4(bb.mn, 0); d.bbmax[i] = f4(bb.mx, 0); }
+}
+B2D_D void refresh_body(const Dev &d, uint32_t i, uint32_t f, v3 pos, q4 orn, float inv_m) {
+    refresh_aabb(d, i, f, pos, orn);
     if (is_dynamic(f)) store_invIW(d, i, world_inertia(orn, load_m3(d.invI, i)), inv_m);
 }
-// integrate_velocities of the bodies outside the island tiles (k_island_tiles integrates its own); with refresh != 0
-// also update_aabbs + update_inertias (solver.cpp:453-465) of every dynamic body, tiled ones included, for when no
-// position iterations run in between.
+// integrate_velocities of the bodies outside the island tiles (k_island_tiles integrates and refreshes its own); with
+// refresh != 0 also update_aabbs + update_inertias (solver.cpp:453-465) of them, for when no position iterations run
+// in between.
 __global__ void __launch_bounds__(256) k_integrate(Dev d, int refresh) {
     if (blockIdx.x == 0 && threadIdx.x == 0) d.cnt->bar = 0;       // grid barrier counter of k_position_df
     GRID_STRIDE(i, d.nbodies) {
         uint32_t f = d.flags[i];
-        if (!is_dynamic(f)) continue;
-        const bool tiled = d.btile[i] != TILE_NONE;
-        if (tiled && !refresh) continue;
+        if (!is_dynamic(f) || d.btile[i] != TILE_NONE) continue;
         float4 p4 = d.pos[i];
         v3 pos = mk3(p4);
         q4 orn = mkq(d.orn[i]);
-        if (!tiled) {
-            v3 v = mk3(d.linvel[i]), w = mk3(d.angvel[i]);
-            integrate_body(v, w, pos, orn, mk3(d.dvw[2 * i]), mk3(d.dvw[2 * i + 1]), d.dt);
-            d.linvel[i] = f4(v, 0); d.angvel[i] = f4(w, 0);
-            d.pos[i] = f4(pos, p4.w); d.orn[i] = f4(orn);
-            d.dvw[2 * i] = make_float4(0, 0, 0, 0); d.dvw[2 * i + 1] = make_float4(0, 0, 0, 0);
-        }
+        v3 v = mk3(d.linvel[i]), w = mk3(d.angvel[i]);
+        integrate_body(v, w, pos, orn, mk3(d.dvw[2 * i]), mk3(d.dvw[2 * i + 1]), d.dt);
+        d.linvel[i] = f4(v, 0); d.angvel[i] = f4(w, 0);
+        d.pos[i] = f4(pos, p4.w); d.orn[i] = f4(orn);
+        d.dvw[2 * i] = make_float4(0, 0, 0, 0); d.dvw[2 * i + 1] = make_float4(0, 0, 0, 0);
         if (refresh) refresh_body(d, i, f, pos, orn, p4.w);
     }
 }
-// refresh_body of the dynamic and kinematic bodies after the position iterations
+// refresh_body of the dynamic and kinematic bodies after the position iterations; k_island_tiles refreshes the tiled ones
 __global__ void __launch_bounds__(256) k_finalize(Dev d) {
     GRID_STRIDE(i, d.nbodies) {
         uint32_t f = d.flags[i];
-        if (kind_of(f) == 2u) continue;
+        if (kind_of(f) == 2u || d.btile[i] != TILE_NONE) continue;
         float4 p4 = d.pos[i];
         refresh_body(d, i, f, mk3(p4), mkq(d.orn[i]), p4.w);
     }
@@ -1689,8 +1681,9 @@ B2D_D void tile_error_max(uint32_t *s_err, uint32_t islot, float err) { if (err 
 // the same records, and positions / orientations / velocities are written once.  One CTA per tile; thread t owns joint t
 // and manifold t of the tile for all iterations, and colours are separated by __syncthreads instead of tickets.  The row,
 // solve, integration and position functions are those of the separate kernels, called in the same order
-// (k_prepare_contacts, k_prepare_hinges, k_integrate, k_store_impulses skip what this kernel has done).  Without position
-// iterations the position loop does not run and the integrated pose is written back.
+// (k_prepare_contacts, k_prepare_hinges, k_integrate, k_store_impulses, k_finalize skip what this kernel has done).  Without
+// position iterations the position loop does not run and the integrated pose is written back.  Either way the AABBs and
+// world-space inverse inertias of the tile's bodies are refreshed from the final pose before it leaves the CTA.
 // Two specialisations of one body (island_tiles<MAXP>), by the most contact points a manifold of the tile may have:
 // k_island_tiles (4) for the generic tiles, k_island_tiles_2p (2) for the two-point tiles, which keep less in registers
 // (ptxas: 40 B of spills at the 128-register cap instead of 280 B; under a 3-CTA bound, 80 registers, it spilled 646 B and
@@ -1789,7 +1782,7 @@ B2D_D void island_tiles(const Dev &d, int vel_iters, int pos_iters) {
             SBody A, B; v3 posA, posB; q4 ornA, ornB; uint32_t sa, sb;
             tile_solver_body(d, s_body, pr.x, A, posA, ornA, sa); tile_solver_body(d, s_body, pr.y, B, posB, ornB, sb);
             // a two-point tile holds no manifold with more points: one that gains a third point sets graph_changed
-            // (k_np_merge) and the rebuild moves its island to a generic tile before the next solve
+            // (np_merge) and the rebuild moves its island to a generic tile before the next solve
             ch = make_uint4(body_tag(pr.x, A), body_tag(pr.y, B), TWO ? min(npts, 2u) : npts, slot_pair(sa, sb));
             contact_point_rows(d, m, A, B, posA, ornA, posB, ornB, a0, a1, a2, a3, aim);
             if (npts > 1) contact_point_rows(d, NM + m, A, B, posA, ornA, posB, ornB, b0, b1, b2, b3, bim);
@@ -1957,9 +1950,16 @@ B2D_D void island_tiles(const Dev &d, int vel_iters, int pos_iters) {
                 d.pA[s * NM + m] = r[0]; d.pN[s * NM + m] = r[2 * TILE_CAP];
             }
         }
+        // the final pose, then update_aabbs + update_inertias of it (k_finalize and k_integrate skip tiled bodies), with
+        // inv_I from records 5-7; the body id is read again from the tile list rather than held across the iterations
         if (t < nb) {
-            const float4 p = s_body[t];
-            d.pos[mybody] = make_float4(p.x, p.y, p.z, d.pos[mybody].w); d.orn[mybody] = s_body[TILE_CAP + t];
+            const uint32_t i = d.tile_body[(size_t)tile * TILE_CAP + t];
+            const float4 p = s_body[t], o = s_body[TILE_CAP + t];
+            const float inv_m = d.pos[i].w;
+            d.pos[i] = make_float4(p.x, p.y, p.z, inv_m); d.orn[i] = o;
+            m3 inv_I; inv_I.r0 = mk3(s_body[5 * TILE_CAP + t]); inv_I.r1 = mk3(s_body[6 * TILE_CAP + t]); inv_I.r2 = mk3(s_body[7 * TILE_CAP + t]);
+            refresh_aabb(d, i, d.flags[i], mk3(p), mkq(o));             // a tiled body is dynamic
+            store_invIW(d, i, world_inertia(mkq(o), inv_I), inv_m);
         }
         __syncthreads();
     }

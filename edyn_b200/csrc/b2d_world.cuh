@@ -135,7 +135,6 @@ struct Dev {
     float4 *pN;        // normal xyz, restitution
     float4 *pL;        // local_normal xyz, bits(att | lifetime << 2)
     float4 *pI;        // normal impulse, friction impulse[2], unused
-    unsigned char *npres;   // narrowphase: number of result points per manifold (points parked in R0/R1/R2)
 
     // ---- islands / colouring
     uint32_t *parent;
