@@ -161,54 +161,64 @@ B2D_D float manifold_score(v3 p0, v3 p1, v3 p2, v3 p3) {                    // g
     return length_sqr(c0) + length_sqr(c1) + length_sqr(c2) + length_sqr(c3);
 }
 
-// geom.cpp:857-985.  Returns the insertion type, writes the index; may increment num_points (append).
-__device__ __noinline__ int insertion_point_index(const v3 *points, int &num_points, v3 np, int &index) {
+// geom.cpp:857-985.  Returns the insertion type, writes the index; may increment num_points (append).  The points
+// come by value (p0..p3; those at and past num_points are not read), so that the manifold merge inlines this with its
+// points in registers; the collide functions call it out of line through insertion_point_index below.
+B2D_D int insertion_index(v3 p0, v3 p1, v3 p2, v3 p3, int &num_points, v3 np, int &index) {
     const float sim = MERGING_THRESHOLD * MERGING_THRESHOLD;
     if (num_points == 0) { index = num_points++; return INS_APPEND; }
     if (num_points == 1) {
-        if (distance_sqr(np, points[0]) > sim) { index = num_points++; return INS_APPEND; }
+        if (distance_sqr(np, p0) > sim) { index = num_points++; return INS_APPEND; }
         index = 0; return INS_SIMILAR;
     }
     if (num_points == 2) {
-        if (length_sqr(cross(np - points[0], np - points[1])) > EPS) { index = num_points++; return INS_APPEND; }
-        float d0 = distance_sqr(np, points[0]), d1 = distance_sqr(np, points[1]), cur = distance_sqr(points[0], points[1]);
+        if (length_sqr(cross(np - p0, np - p1)) > EPS) { index = num_points++; return INS_APPEND; }
+        float d0 = distance_sqr(np, p0), d1 = distance_sqr(np, p1), cur = distance_sqr(p0, p1);
         if (d0 > cur && d0 > d1) { index = 1; return d1 < sim ? INS_SIMILAR : INS_REPLACE; }
         if (d1 > cur && d1 > d0) { index = 0; return d0 < sim ? INS_SIMILAR : INS_REPLACE; }
         index = 4; return INS_NONE;
     }
     if (num_points == 3) {
-        v3 normal = cross(points[0] - points[1], points[1] - points[2]);
+        v3 normal = cross(p0 - p1, p1 - p2);
         if (try_normalize(normal)) {
-            if (fabsf(dot(np - points[0], normal)) < EPS && point_in_triangle(points[0], points[1], points[2], normal, np)) {
+            if (fabsf(dot(np - p0, normal)) < EPS && point_in_triangle(p0, p1, p2, normal, np)) {
                 index = 4; return INS_NONE;
             }
             index = num_points++; return INS_APPEND;
         }
-        float d0 = dot(points[1] - points[0], points[2] - points[0]);
+        float d0 = dot(p1 - p0, p2 - p0);
         if (d0 > 0 && d0 < 1) { index = 1; return INS_REPLACE; }
-        float d1 = dot(points[0] - points[1], points[2] - points[1]);
+        float d1 = dot(p0 - p1, p2 - p1);
         if (d1 > 0 && d1 < 1) { index = 0; return INS_REPLACE; }
-        float d2 = dot(points[2] - points[0], points[1] - points[0]);
+        float d2 = dot(p2 - p0, p1 - p0);
         if (d2 > 0 && d2 < 1) { index = 2; return INS_REPLACE; }
-        float ds0 = distance_sqr(points[0], points[1]), ds1 = distance_sqr(points[1], points[2]), ds2 = distance_sqr(points[2], points[0]);
+        float ds0 = distance_sqr(p0, p1), ds1 = distance_sqr(p1, p2), ds2 = distance_sqr(p2, p0);
         int mi = -1; float md = SCALAR_MAX;
         if (ds0 < md) { md = ds0; mi = 0; }
         if (ds1 < md) { md = ds1; mi = 1; }
         if (ds2 < md) { md = ds2; mi = 2; }
         index = mi; return INS_REPLACE;       // mi == -1 only for NaN input, as SIZE_MAX in the reference
     }
-    float sc0 = manifold_score(np, points[1], points[2], points[3]);
-    float sc1 = manifold_score(np, points[0], points[2], points[3]);
-    float sc2 = manifold_score(np, points[0], points[1], points[3]);
-    float sc3 = manifold_score(np, points[0], points[1], points[2]);
-    float max_score = manifold_score(points[0], points[1], points[2], points[3]);
+    float sc0 = manifold_score(np, p1, p2, p3);
+    float sc1 = manifold_score(np, p0, p2, p3);
+    float sc2 = manifold_score(np, p0, p1, p3);
+    float sc3 = manifold_score(np, p0, p1, p2);
+    float max_score = manifold_score(p0, p1, p2, p3);
     int mi = -1;
     if (sc0 > max_score) { max_score = sc0; mi = 0; }
     if (sc1 > max_score) { max_score = sc1; mi = 1; }
     if (sc2 > max_score) { max_score = sc2; mi = 2; }
     if (sc3 > max_score) { max_score = sc3; mi = 3; }
-    if (mi >= 0) { index = mi; return distance_sqr(points[mi], np) < sim ? INS_SIMILAR : INS_REPLACE; }
+    if (mi >= 0) {
+        const v3 pm = mi == 0 ? p0 : mi == 1 ? p1 : mi == 2 ? p2 : p3;
+        index = mi; return distance_sqr(pm, np) < sim ? INS_SIMILAR : INS_REPLACE;
+    }
     index = 4; return INS_NONE;
+}
+__device__ __noinline__ int insertion_point_index(const v3 *points, int &num_points, v3 np, int &index) {
+    const int n = num_points;
+    return insertion_index(n > 0 ? points[0] : np, n > 1 ? points[1] : np, n > 2 ? points[2] : np, n > 3 ? points[3] : np,
+                           num_points, np, index);
 }
 
 B2D_D void add_point(CResult &r, const CPoint &p) { r.pt[r.num++] = p; }     // collision_result.cpp:6-10

@@ -404,6 +404,7 @@ B2D_D unsigned lbits(float4 pl) { return __float_as_uint(pl.w); }
 B2D_D int find_nearest_contact(v3 cpA, v3 cpB, const CResult &res) {
     float shortest = CACHING_THRESHOLD * CACHING_THRESHOLD;
     int nearest = res.num;
+    #pragma unroll 1
     for (int i = 0; i < res.num; ++i) {
         float dA = length_sqr(res.pt[i].pivotA - cpA);
         float dB = length_sqr(res.pt[i].pivotB - cpB);
@@ -426,24 +427,23 @@ B2D_D int find_nearest_contact_rolling(const CResult &res, v3 cp_pivot, v3 origi
     return nearest;
 }
 
-struct MPoint {   // one persisted contact point in registers
+// One contact point in registers, without its warm-start impulse: pI is only touched where a point changes slots or
+// is created (np_merge), so a point that stays where it is keeps its impulse without a load or a store.
+struct MPoint {
     v3 pivotA, pivotB, normal, local_normal;
     float distance, friction, restitution;
     unsigned att, lifetime;
-    v3 imp;
 };
 B2D_D void load_point(const Dev &d, uint32_t m, int s, MPoint &p) {
     size_t i = (size_t)s * d.NM + m;
-    float4 a = d.pA[i], b = d.pB[i], n = d.pN[i], l = d.pL[i], im = d.pI[i];
+    float4 a = d.pA[i], b = d.pB[i], n = d.pN[i], l = d.pL[i];
     p.pivotA = mk3(a); p.distance = a.w; p.pivotB = mk3(b); p.friction = b.w; p.normal = mk3(n); p.restitution = n.w;
     p.local_normal = mk3(l); unsigned u = __float_as_uint(l.w); p.att = u & 3u; p.lifetime = u >> 2;
-    p.imp = mk3(im);
 }
 B2D_D void store_point(const Dev &d, uint32_t m, int s, const MPoint &p) {
     size_t i = (size_t)s * d.NM + m;
     d.pA[i] = f4(p.pivotA, p.distance); d.pB[i] = f4(p.pivotB, p.friction); d.pN[i] = f4(p.normal, p.restitution);
     d.pL[i] = f4(p.local_normal, __uint_as_float((p.att & 3u) | (p.lifetime << 2)));
-    d.pI[i] = f4(p.imp, 0);
 }
 // merge_point, collision_util.cpp:205-231
 B2D_D void merge_point(const CPoint &rp, MPoint &cp, q4 ornA, q4 ornB) {
@@ -459,8 +459,12 @@ B2D_D MPoint create_point(const CPoint &rp, q4 ornA, q4 ornB, float2 matA, float
     else cp.local_normal = mk3(0, 0, 0);
     cp.friction = sqrtf(matA.x * matB.x);
     cp.restitution = fminf(matA.y, matB.y);
-    cp.lifetime = 0; cp.imp = mk3(0, 0, 0);
+    cp.lifetime = 0;
     return cp;
+}
+B2D_D int nth_set_bit(unsigned mask, int n) {          // position of the n-th (from 0) set bit of mask
+    for (int k = 0; k < n; ++k) mask &= mask - 1u;
+    return __ffs(mask) - 1;
 }
 
 // Narrowphase in three steps:
@@ -525,83 +529,118 @@ __global__ void __launch_bounds__(256) k_np_scatter(Dev d) {
 }
 
 // update_contact_distances (collision_util.cpp:28-45) + process_collision (collision_util.hpp:105-276, sequential flavour
-// of narrowphase.hpp:62-84) of alive, awake manifold m in state st between bodies pr.x (flags fa, pose posA ornA) and
-// pr.y, with this step's collision result res
-B2D_D void np_merge(const Dev &d, uint32_t m, uint32_t st, uint2 pr, uint32_t fa, uint32_t fb,
-                    v3 posA, q4 ornA, v3 posB, q4 ornB, const CResult &res) {
-    int num = (int)(st & MS_NPTS_MASK);
-    if (num == 0 && res.num == 0) return;
-    const uint32_t a = pr.x, b = pr.y;
-    MPoint P[4];
-    for (int s = 0; s < num; ++s) {
-        load_point(d, m, s, P[s]);
-        v3 pAw = to_world(P[s].pivotA, posA, ornA), pBw = to_world(P[s].pivotB, posB, ornB);
-        P[s].distance = dot(P[s].normal, pAw - pBw);
+// of narrowphase.hpp:62-84) of alive, awake manifold m with this step's collision result res.  The manifold's state and
+// pair and the bodies' flags and poses are read here, after the collision, rather than held in registers across it.
+//
+// No per-point array: the state of the (at most 4) points is kept in bit fields, the points themselves in their slots
+// in HBM, so nothing here is indexed at run time but res, and the merge adds nothing to the local frame.  Each persisted
+// point is updated in its own slot as soon as it is processed.  When every point stays and every result point merged
+// into one -- the settled case -- that is all.  Otherwise np_rearrange moves the points into the reference's order.
+//
+// np_rearrange: the rest of process_collision once the persisted points are merged and stored in place.  `keep` says
+// which slots hold a point that stays, `merged` which result points a persisted point took.  Inserts the other result
+// points and writes the final list, newest first and capped at 4, moving impulses with the points; returns its length.
+B2D_D int np_rearrange(const Dev &d, uint32_t m, uint2 pr, const CResult &res, unsigned keep, unsigned merged) {
+    const int num = __popc(keep);       // the persisted list after the removals: its point j sits in slot nth_set_bit(keep, j)
+    // ---- insertion.  L is the persisted list with the result points written over it: slot j of L is persisted point
+    //      j while type j is INS_NONE, else result point lsrc j (2 bits per slot in `type` and `lsrc`)
+    int num_points = num;
+    unsigned type = 0u, lsrc = 0u;
+    if (merged != (1u << res.num) - 1u) {
+        if (num_points == 0) { num_points = 1; type = INS_APPEND; merged |= 1u; }
+        auto piv = [&](int j, bool B) -> v3 {           // pivot A or B of slot j of L
+            if (j >= num_points) return mk3(0, 0, 0);   // not read by insertion_index
+            if (type >> 2 * j & 3u) { const CPoint &q = res.pt[lsrc >> 2 * j & 3u]; return B ? q.pivotB : q.pivotA; }
+            const size_t i = (size_t)nth_set_bit(keep, j) * d.NM + m;
+            return mk3(B ? d.pB[i] : d.pA[i]);
+        };
+        #pragma unroll 1
+        for (int k = 0; k < res.num; ++k) {
+            if (merged >> k & 1u) continue;
+            int idx, t = INS_NONE;
+            #pragma unroll 1
+            for (int B = 0; B < 2 && t == INS_NONE; ++B)          // pivots A, then pivots B if A found no place
+                t = insertion_index(piv(0, B), piv(1, B), piv(2, B), piv(3, B), num_points, B ? res.pt[k].pivotB : res.pt[k].pivotA, idx);
+            if (t != INS_NONE && idx >= 0 && idx < 4) {
+                type = (type & ~(3u << 2 * idx)) | (unsigned)t << 2 * idx;
+                lsrc = (lsrc & ~(3u << 2 * idx)) | (unsigned)k << 2 * idx;
+            }
+        }
     }
-    // ---- merge with persisted points
-    bool merged[4] = {false, false, false, false};
+    // ---- the slots of L that become new points (appended, similar to no persisted point, or replacing one), and the
+    //      persisted points that stay alive
+    unsigned created = 0u, alive = (1u << num) - 1u;
+    for (int j = 0; j < num_points; ++j) {
+        const unsigned t = type >> 2 * j & 3u;
+        if (t == INS_APPEND || t == INS_REPLACE || (t == INS_SIMILAR && j >= num)) created |= 1u << j;
+        if (t == INS_REPLACE && j < num) alive &= ~(1u << j);
+    }
+    const int n_created = __popc(created);
+    // ---- the list: the created points newest first, then the alive persisted points in order, at most 4.  Persisted
+    //      point j moves from slot s to slot n_created + (alive points before it); both grow with j, so the points that
+    //      move up go first, last point first, then the rest in order, and no point is overwritten before it moved
+    auto place = [&](int j, bool up) {
+        if (!(alive >> j & 1u)) return;
+        const int s = nth_set_bit(keep, j), dst = n_created + __popc(alive & ((1u << j) - 1u));
+        const bool similar = (type >> 2 * j & 3u) == INS_SIMILAR;
+        if (dst >= MAX_CONTACTS || (dst > s) != up || (dst == s && !similar)) return;
+        MPoint cp;
+        load_point(d, m, s, cp);
+        if (similar) merge_point(res.pt[lsrc >> 2 * j & 3u], cp, mkq(d.orn[pr.x]), mkq(d.orn[pr.y]));
+        store_point(d, m, dst, cp);
+        if (dst != s) d.pI[(size_t)dst * d.NM + m] = f4(mk3(d.pI[(size_t)s * d.NM + m]), 0);
+    };
+    #pragma unroll 1
+    for (int j = num - 1; j >= 0; --j) place(j, true);
+    #pragma unroll 1
+    for (int j = 0; j < num; ++j) place(j, false);
+    if (created) {
+        const float2 matA = d.mat[pr.x], matB = d.mat[pr.y];
+        const q4 ornA = mkq(d.orn[pr.x]), ornB = mkq(d.orn[pr.y]);
+        int dst = n_created;
+        #pragma unroll 1
+        for (int j = 0; j < num_points; ++j) {
+            if (!(created >> j & 1u)) continue;
+            store_point(d, m, --dst, create_point(res.pt[lsrc >> 2 * j & 3u], ornA, ornB, matA, matB));
+            d.pI[(size_t)dst * d.NM + m] = make_float4(0, 0, 0, 0);
+        }
+    }
+    return min(MAX_CONTACTS, n_created + __popc(alive));
+}
+B2D_D void np_merge(const Dev &d, uint32_t m, const CResult &res) {
+    const uint32_t st = d.mstate[m];
+    const uint2 pr = d.mpair[m];
+    const int num0 = (int)(st & MS_NPTS_MASK);
+    if (num0 == 0 && res.num == 0) return;
+    const uint32_t a = pr.x, b = pr.y, fa = d.flags[a], fb = d.flags[b];
+    const v3 posA = mk3(d.pos[a]), posB = mk3(d.pos[b]);
+    const q4 ornA = mkq(d.orn[a]), ornB = mkq(d.orn[b]);
+    // ---- merge with persisted points, in their order.  The reference erases a removed point from its list, which
+    //      shifts the later ones down; here it clears the point's bit in `keep`, and np_rearrange closes the gap.
+    unsigned merged = 0u, keep = 0u;        // bit k: res.pt[k] was merged into a point; bit s: the point of slot s stays
     const bool rollA = fa & F_ROLLING, rollB = fb & F_ROLLING;
-    int i = 0;
-    while (i < num) {
-        MPoint &cp = P[i];
+    #pragma unroll 1
+    for (int s = 0; s < num0; ++s) {
+        MPoint cp;
+        load_point(d, m, s, cp);
         ++cp.lifetime;
         int nearest = find_nearest_contact(cp.pivotA, cp.pivotB, res);
         if (nearest == res.num && rollA) nearest = find_nearest_contact_rolling(res, cp.pivotA, posA, ornA, mk3(d.angvel[a]), d.dt);
         if (nearest == res.num && rollB) nearest = find_nearest_contact_rolling(res, cp.pivotB, posB, ornB, mk3(d.angvel[b]), d.dt);
-        bool remove = false;
-        if (nearest < res.num && !merged[nearest]) { merge_point(res.pt[nearest], cp, ornA, ornB); merged[nearest] = true; }
+        if (nearest < res.num && !(merged >> nearest & 1u)) { merge_point(res.pt[nearest], cp, ornA, ornB); merged |= 1u << nearest; }
         else {                                          // should_remove_point, collision_util.cpp:397-413
             v3 pA = to_world(cp.pivotA, posA, ornA), pB = to_world(cp.pivotB, posB, ornB);
             v3 dd = pA - pB;
             float nd = dot(dd, cp.normal);
             v3 td = dd - nd * cp.normal;
-            remove = nd > BREAKING_THRESHOLD || length_sqr(td) > BREAKING_THRESHOLD * BREAKING_THRESHOLD;
+            if (nd > BREAKING_THRESHOLD || length_sqr(td) > BREAKING_THRESHOLD * BREAKING_THRESHOLD) continue;
+            cp.distance = dot(cp.normal, pA - pB);      // update_contact_distances
         }
-        if (remove) { for (int k = i + 1; k < num; ++k) P[k - 1] = P[k]; --num; }
-        else ++i;
+        keep |= 1u << s;
+        store_point(d, m, s, cp);
     }
-    bool all = true;
-    for (int k = 0; k < res.num; ++k) all = all && merged[k];
-    if (!all) {
-        CPoint L[4]; int ent[4] = {-1, -1, -1, -1}; int type[4] = {INS_NONE, INS_NONE, INS_NONE, INS_NONE};
-        int num_points = num;
-        if (num_points > 0) {
-            for (int k = 0; k < num; ++k) { L[k].pivotA = P[k].pivotA; L[k].pivotB = P[k].pivotB; L[k].normal = P[k].normal; L[k].distance = P[k].distance; L[k].att = ATT_NONE; ent[k] = k; }
-        } else {
-            num_points = 1; L[0] = res.pt[0]; type[0] = INS_APPEND; merged[0] = true;
-        }
-        for (int k = 0; k < res.num; ++k) {
-            if (merged[k]) continue;
-            v3 piv[4];
-            for (int j = 0; j < num_points; ++j) piv[j] = L[j].pivotA;
-            int idx;
-            int t = insertion_point_index(piv, num_points, res.pt[k].pivotA, idx);
-            if (t == INS_NONE) {
-                for (int j = 0; j < num_points; ++j) piv[j] = L[j].pivotB;
-                t = insertion_point_index(piv, num_points, res.pt[k].pivotB, idx);
-            }
-            if (t != INS_NONE && idx >= 0 && idx < 4) { L[idx] = res.pt[k]; type[idx] = t; }
-        }
-        const float2 matA = d.mat[a], matB = d.mat[b];
-        MPoint created[4]; int n_created = 0;
-        bool alive[4] = {true, true, true, true};
-        for (int k = 0; k < num_points; ++k) {
-            if (type[k] == INS_APPEND) created[n_created++] = create_point(L[k], ornA, ornB, matA, matB);
-            else if (type[k] == INS_SIMILAR) {
-                if (ent[k] < 0) created[n_created++] = create_point(L[k], ornA, ornB, matA, matB);
-                else merge_point(L[k], P[ent[k]], ornA, ornB);
-            } else if (type[k] == INS_REPLACE) {
-                if (ent[k] >= 0) alive[ent[k]] = false;
-                created[n_created++] = create_point(L[k], ornA, ornB, matA, matB);
-            }
-        }
-        MPoint Q[4]; int w = 0;
-        for (int k = n_created - 1; k >= 0; --k) Q[w++] = created[k];      // newest point = list head
-        for (int k = 0; k < num; ++k) if (alive[k] && w < 4) Q[w++] = P[k];
-        num = w;
-        for (int k = 0; k < num; ++k) P[k] = Q[k];
-    }
-    for (int s = 0; s < num; ++s) store_point(d, m, s, P[s]);
+    int num = __popc(keep);
+    if (keep != (1u << num0) - 1u || merged != (1u << res.num) - 1u) num = np_rearrange(d, m, pr, res, keep, merged);
     d.mstate[m] = (st & ~MS_NPTS_MASK) | (uint32_t)num;
     // the island rebuild reads whether a manifold has points (colouring, island census) and, on the dataflow path,
     // its point count (sort key); inside an island tile the count only matters to the solver itself, except that a
@@ -644,16 +683,18 @@ B2D_D void np_manifold(const Dev &d, uint32_t i) {
             swap_result(res);
         }
     }
-    np_merge(d, m, st, pr, fa, fb, posA, ornA, posB, ornB, res);
+    np_merge(d, m, res);
 }
-// the two heavy overloads (box-box, capsule-box) get a launch each over their range of the list
+// the two heavy overloads (box-box, capsule-box) get a launch each over their range of the list.  The launch bounds
+// hold the residency the collide code needs (3, 4 and, for the light kernel, 6 CTAs per SM), so that the merge's
+// cold insertion path does not raise the register count for everyone
 template <int FN>
-__global__ void __launch_bounds__(128) k_np_collide(Dev d) {
+__global__ void __launch_bounds__(128, FN == 5 ? 3 : 4) k_np_collide(Dev d) {
     const uint32_t b = d.cnt->npoff[FN], e = d.cnt->npoff[FN + 1];
     for (uint32_t i = b + blockIdx.x * blockDim.x + threadIdx.x; i < e; i += gridDim.x * blockDim.x) np_manifold<FN>(d, i);
 }
 // the seven light ones share one: types 1-4 and 6-8, two ranges of the list walked as one
-__global__ void __launch_bounds__(128) k_np_collide_light(Dev d) {
+__global__ void __launch_bounds__(128, 6) k_np_collide_light(Dev d) {
     const uint32_t b0 = d.cnt->npoff[1], n0 = d.cnt->npoff[5] - b0, b1 = d.cnt->npoff[6], n = n0 + d.cnt->npoff[9] - b1;
     for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) np_manifold<0>(d, j < n0 ? b0 + j : b1 + (j - n0));
 }
