@@ -1032,6 +1032,11 @@ int b2d_upload_contacts(b2d_world *w, uint32_t n, const uint32_t *pairs, const u
     for (uint32_t k = 0; k < n; ++k) {
         pr[k] = make_uint2(pairs[2 * k], pairs[2 * k + 1]);
         if (num[k] > 4) { w->error = "b2d_upload_contacts: more than 4 points"; return B2D_ERR_ARGUMENT; }
+        for (uint32_t s = 0; s < num[k]; ++s) {      // the point layout packs attachment | lifetime << 2 into one word
+            const uint32_t *u = ptu2 + ((size_t)k * 4 + s) * 2;
+            if (u[0] > 2u) { w->error = "b2d_upload_contacts: normal_attachment > 2"; return B2D_ERR_ARGUMENT; }
+            if (u[1] >= (1u << 30)) { w->error = "b2d_upload_contacts: lifetime >= 2^30"; return B2D_ERR_ARGUMENT; }
+        }
         st[k] = MS_ALIVE | (COLOR_NONE << MS_COLOR_SHIFT) | num[k];
         for (uint32_t s = 0; s < 4; ++s) {
             const float *f = pt18 + ((size_t)k * 4 + s) * 18; const uint32_t *u = ptu2 + ((size_t)k * 4 + s) * 2;

@@ -170,7 +170,10 @@ int b2d_download_state(b2d_world *w, float *pos, float *orn, float *linvel, floa
 /* Contact manifolds (contact_manifold / contact_point*, include/edyn/collision/contact_point.hpp:17-58).
  * pairs: 2 uint32 per manifold (body[0], body[1]).  num: points per manifold.  Per point slot
  * (4 per manifold, list order, slot 0 = newest): pt18 = pivotA(3) pivotB(3) normal(3) local_normal(3)
- * distance friction restitution normal_impulse friction_impulse[2]; pt_u2 = {normal_attachment, lifetime}. */
+ * distance friction restitution normal_impulse friction_impulse[2]; pt_u2 = {normal_attachment, lifetime}.
+ * A point stores its attachment and lifetime in one 32-bit word: b2d_upload_contacts returns B2D_ERR_ARGUMENT for a
+ * normal_attachment > 2 or a lifetime >= 2^30 in any of the first num slots.  The step counts a lifetime modulo 2^30
+ * (about 207 days at 60 Hz) where the reference's uint32 would go on; nothing in the step reads it. */
 int b2d_num_manifolds(b2d_world *w, uint32_t *n);
 int b2d_download_pairs(b2d_world *w, uint32_t capacity, uint32_t *pairs, uint32_t *n);
 int b2d_download_contacts(b2d_world *w, uint32_t capacity, uint32_t *pairs, uint32_t *num,

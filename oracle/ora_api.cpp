@@ -159,6 +159,16 @@ void ora_get_contacts(void *h, uint32_t *num, float *pt18, uint32_t *pt_u2) {
     }
 }
 
+// Merge trace (ora_world.hpp, merge_branch): on = record it in every following narrowphase; get: one word per manifold
+// from the last one (zeros where it was off).  Returns the number of words, or MB_COUNT when out is null.
+void ora_set_merge_trace(void *h, int on) { static_cast<World *>(h)->trace_merge = on != 0; }
+uint32_t ora_get_merge_trace(void *h, uint64_t *out) {
+    World &w = *static_cast<World *>(h);
+    if (!out) return MB_COUNT;
+    for (size_t i = 0; i < w.manifolds.size(); ++i) out[i] = i < w.merge_trace.size() ? w.merge_trace[i] : 0;
+    return uint32_t(w.manifolds.size());
+}
+
 // Replace all manifolds (solver-only / narrowphase-only tests).  Same layout as ora_get_contacts.
 void ora_set_contacts(void *h, uint32_t n, const uint32_t *pairs, const uint32_t *num, const float *pt18, const uint32_t *pt_u2) {
     World &w = *static_cast<World *>(h);

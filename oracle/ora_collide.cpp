@@ -190,7 +190,7 @@ static scalar manifold_score(vec3 p0, vec3 p1, vec3 p2, vec3 p3) {
 }
 
 // src/edyn/math/geom.cpp:857-985
-insert_res insertion_point_index(const vec3 *points, size_t count, size_t &num_points, vec3 new_point) {
+insert_res insertion_point_index(const vec3 *points, size_t count, size_t &num_points, vec3 new_point, int *collinear) {
     const scalar max_dist_similar_sqr = MERGING_THRESHOLD * MERGING_THRESHOLD;
     if (num_points == 0) return {INS_APPEND, num_points++};
     if (num_points == 1) {
@@ -218,11 +218,12 @@ insert_res insertion_point_index(const vec3 *points, size_t count, size_t &num_p
             return {INS_APPEND, num_points++};
         }
         scalar d0 = dot(points[1] - points[0], points[2] - points[0]);
-        if (d0 > 0 && d0 < 1) return {INS_REPLACE, 1};
+        if (d0 > 0 && d0 < 1) { if (collinear) *collinear = 0; return {INS_REPLACE, 1}; }
         scalar d1 = dot(points[0] - points[1], points[2] - points[1]);
-        if (d1 > 0 && d1 < 1) return {INS_REPLACE, 0};
+        if (d1 > 0 && d1 < 1) { if (collinear) *collinear = 1; return {INS_REPLACE, 0}; }
         scalar d2 = dot(points[2] - points[0], points[1] - points[0]);
-        if (d2 > 0 && d2 < 1) return {INS_REPLACE, 2};
+        if (d2 > 0 && d2 < 1) { if (collinear) *collinear = 2; return {INS_REPLACE, 2}; }
+        if (collinear) *collinear = 3;
         scalar ds[3] = {distance_sqr(points[0], points[1]), distance_sqr(points[1], points[2]),
                         distance_sqr(points[2], points[0])};
         size_t mi = SIZE_MAX; scalar md = SCALAR_MAX;

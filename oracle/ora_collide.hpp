@@ -48,7 +48,8 @@ scalar closest_point_segment_segment(vec3 p1, vec3 q1, vec3 p2, vec3 q2, scalar 
                                      vec3 &c1, vec3 &c2, size_t *num_points = nullptr,
                                      scalar *sp = nullptr, scalar *tp = nullptr,
                                      vec3 *c1p = nullptr, vec3 *c2p = nullptr);
-insert_res insertion_point_index(const vec3 *points, size_t count, size_t &num_points, vec3 new_point);
+// collinear (optional, merge tests): which branch of the collinear three-point case decided, 0-3 = d0, d1, d2, shortest edge
+insert_res insertion_point_index(const vec3 *points, size_t count, size_t &num_points, vec3 new_point, int *collinear = nullptr);
 void maybe_add_point(cresult &r, const cpoint &np);
 
 // box feature helpers (src/edyn/shapes/box_shape.cpp)

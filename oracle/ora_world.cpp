@@ -273,15 +273,15 @@ void World::broadphase() {
 
 // ------------------------------------------------------------------ narrowphase
 
-// src/edyn/util/collision_util.cpp:233-255
-size_t find_nearest_contact(const Point &cp, const cresult &res) {
+// src/edyn/util/collision_util.cpp:233-255; *via_B (merge trace): the nearest point won through pivot B
+size_t find_nearest_contact(const Point &cp, const cresult &res, bool *via_B) {
     scalar shortest = square(CACHING_THRESHOLD);
     size_t nearest = res.num;
     for (size_t i = 0; i < res.num; ++i) {
         scalar dA = length_sqr(res.pt[i].pivotA - cp.pivotA);
         scalar dB = length_sqr(res.pt[i].pivotB - cp.pivotB);
-        if (dA < shortest) { shortest = dA; nearest = i; }
-        if (dB < shortest) { shortest = dB; nearest = i; }
+        if (dA < shortest) { shortest = dA; nearest = i; if (via_B) *via_B = false; }
+        if (dB < shortest) { shortest = dB; nearest = i; if (via_B) *via_B = true; }
     }
     return nearest;
 }
@@ -331,30 +331,64 @@ static Point create_point(const cpoint &rp, const Body &A, const Body &B) {
 }
 
 // include/edyn/util/collision_util.hpp:105-276, sequential flavour (narrowphase.hpp:62-84): points are
-// destroyed/created immediately; new points are pushed at the head of the manifold's list.
-static void process_collision(Manifold &m, const cresult &res, const Body &A, const Body &B, scalar dt) {
+// destroyed/created immediately; new points are pushed at the head of the manifold's list.  tr (may be null): the
+// merge_branch bits this call took.
+static void process_collision(Manifold &m, const cresult &res, const Body &A, const Body &B, scalar dt, uint64_t *tr) {
+    uint64_t t = 0;
+    auto hit = [&](uint32_t b) { t |= uint64_t(1) << b; };
     bool merged[4] = {false, false, false, false};
+    const size_t num0 = m.num;
+    uint32_t slot[4] = {0, 1, 2, 3};                 // the slot each point of the list sat in when the step started
+    unsigned removed = 0;                            // by slot
     size_t i = 0;
     while (i < m.num) {
         Point &cp = m.pt[i];
         ++cp.lifetime;
-        size_t nearest = find_nearest_contact(cp, res);
-        if (nearest == res.num && A.rolling) nearest = find_nearest_contact_rolling(res, cp.pivotA, A.pos, A.orn, A.angvel, dt);
-        if (nearest == res.num && B.rolling) nearest = find_nearest_contact_rolling(res, cp.pivotB, B.pos, B.orn, B.angvel, dt);
+        bool via_B = false;
+        size_t nearest = find_nearest_contact(cp, res, &via_B);
+        uint32_t how = via_B ? MB_NEAREST_B : MB_NEAREST_A;
+        if (nearest == res.num && A.rolling) { nearest = find_nearest_contact_rolling(res, cp.pivotA, A.pos, A.orn, A.angvel, dt); how = MB_ROLL_A; }
+        if (nearest == res.num && B.rolling) {
+            if (A.rolling) hit(MB_ROLL_BOTH);
+            nearest = find_nearest_contact_rolling(res, cp.pivotB, B.pos, B.orn, B.angvel, dt); how = MB_ROLL_B;
+        }
         if (nearest < res.num && !merged[nearest]) {
+            hit(how);
             merge_point(res.pt[nearest], cp, A.orn, B.orn);
             merged[nearest] = true;
             ++i;
-        } else if (should_remove_point(cp, A.pos, A.orn, B.pos, B.orn)) {
-            for (size_t k = i + 1; k < m.num; ++k) m.pt[k - 1] = m.pt[k];
+            continue;
+        }
+        if (nearest < res.num) hit(MB_TAKEN);
+        if (should_remove_point(cp, A.pos, A.orn, B.pos, B.orn)) {
+            const vec3 d = to_world(cp.pivotA, A.pos, A.orn) - to_world(cp.pivotB, B.pos, B.orn);
+            hit(dot(d, cp.normal) > BREAKING_THRESHOLD ? MB_REMOVE_NORMAL : MB_REMOVE_TANGENT);
+            removed |= 1u << slot[i];
+            for (size_t k = i + 1; k < m.num; ++k) { m.pt[k - 1] = m.pt[k]; slot[k - 1] = slot[k]; }
             --m.num;
         } else {
+            hit(MB_KEPT);
             ++i;
         }
     }
+    if (num0 == 0 && res.num == 0) hit(MB_EARLY_RETURN);
+    if (res.num == 0 && m.num > 0) hit(MB_EMPTY_KEEP);
+    if (res.num == 0 && removed) hit(MB_EMPTY_REMOVE);
+    if (removed && num0 >= 2) {
+        if (removed & 1u) hit(MB_REMOVE_FIRST);
+        if (removed >> (num0 - 1) & 1u) hit(MB_REMOVE_LAST);
+        if (removed & ((1u << (num0 - 1)) - 1u) & ~1u) hit(MB_REMOVE_MIDDLE);
+        for (size_t k = 1; k + 1 < num0; ++k)
+            if (!(removed >> k & 1u) && (removed & ((1u << k) - 1u)) && (removed >> (k + 1))) hit(MB_REMOVE_GAP);
+        if (num0 == 4 && removed == 15u) hit(MB_REMOVE_ALL4);
+    }
     bool all = true;
     for (size_t k = 0; k < res.num; ++k) all = all && merged[k];
-    if (all) return;
+    if (all) {
+        if (num0 > 0 && res.num > 0 && !removed) hit(MB_SETTLED);
+        if (tr) *tr = t;
+        return;
+    }
 
     struct Local { cpoint p; int ent; insert_type type; };
     Local L[4];
@@ -371,19 +405,38 @@ static void process_collision(Manifold &m, const cresult &res, const Body &A, co
         L[0].type = INS_APPEND;
         merged[0] = true;
     }
+    // insertion_point_index with the branch it took recorded
+    auto insert = [&](const vec3 *pivots, vec3 p) {
+        const size_t n = num_points;
+        int col = -1;
+        const insert_res ir = insertion_point_index(pivots, 4, num_points, p, &col);
+        static const uint32_t b1[4] = {MB_COUNT, MB_INS1_SIMILAR, MB_COUNT, MB_INS1_APPEND};
+        static const uint32_t b3[4] = {MB_INS3_COL1, MB_INS3_COL0, MB_INS3_COL2, MB_INS3_SHORTEST};
+        if (n == 1) hit(b1[ir.type]);
+        else if (n == 2) hit(ir.type == INS_APPEND ? MB_INS2_APPEND : ir.type == INS_SIMILAR ? MB_INS2_SIMILAR
+                             : ir.type == INS_REPLACE ? MB_INS2_REPLACE0 + uint32_t(ir.index) : MB_INS2_NONE);
+        else if (n == 3) hit(ir.type == INS_NONE ? MB_INS3_NONE : ir.type == INS_APPEND ? MB_INS3_APPEND : b3[col]);
+        else if (n == 4) hit(ir.type == INS_SIMILAR ? MB_INS4_SIMILAR : ir.type == INS_REPLACE ? MB_INS4_REPLACE0 + uint32_t(ir.index) : MB_INS4_NONE);
+        return ir;
+    };
     for (size_t k = 0; k < res.num; ++k) {
         if (merged[k]) continue;
         const cpoint &rp = res.pt[k];
         vec3 pivots[4];
         for (size_t j = 0; j < num_points; ++j) pivots[j] = L[j].p.pivotA;
-        insert_res ir = insertion_point_index(pivots, 4, num_points, rp.pivotA);
+        insert_res ir = insert(pivots, rp.pivotA);
         if (ir.type == INS_NONE) {
             for (size_t j = 0; j < num_points; ++j) pivots[j] = L[j].p.pivotB;
-            ir = insertion_point_index(pivots, 4, num_points, rp.pivotB);
+            ir = insert(pivots, rp.pivotB);
+            if (ir.type != INS_NONE) hit(MB_PIVOT_B);
         }
-        if (ir.type != INS_NONE) { L[ir.index].p = rp; L[ir.index].type = ir.type; }
+        if (ir.type != INS_NONE) {
+            if (L[ir.index].type == INS_REPLACE && ir.type == INS_SIMILAR) hit(MB_REPLACE_THEN_SIMILAR);
+            if (L[ir.index].type == INS_SIMILAR && ir.type == INS_REPLACE) hit(MB_SIMILAR_THEN_REPLACE);
+            L[ir.index].p = rp; L[ir.index].type = ir.type;
+        }
     }
-    Point existing[4]; bool alive[4] = {false, false, false, false};
+    Point existing[4]; bool alive[4] = {false, false, false, false}, similar[4] = {false, false, false, false};
     const size_t n_exist = m.num;
     for (size_t k = 0; k < n_exist; ++k) { existing[k] = m.pt[k]; alive[k] = true; }
     Point created[4]; size_t n_created = 0;
@@ -393,22 +446,36 @@ static void process_collision(Manifold &m, const cresult &res, const Body &A, co
         case INS_NONE: break;
         case INS_APPEND: created[n_created++] = create_point(l.p, A, B); break;
         case INS_SIMILAR:
-            if (l.ent < 0) created[n_created++] = create_point(l.p, A, B);
-            else merge_point(l.p, existing[l.ent], A.orn, B.orn);
+            if (l.ent < 0) { hit(MB_SIMILAR_CREATED); created[n_created++] = create_point(l.p, A, B); }
+            else { similar[l.ent] = true; merge_point(l.p, existing[l.ent], A.orn, B.orn); }
             break;
         case INS_REPLACE:
-            if (l.ent >= 0) alive[l.ent] = false;
+            if (l.ent >= 0) {
+                hit(MB_REPLACE_PERSISTED);
+                if (slot[l.ent] != uint32_t(l.ent)) hit(MB_REPLACE_AFTER_GAP);
+                alive[l.ent] = false;
+            }
             created[n_created++] = create_point(l.p, A, B);
             break;
         }
     }
     size_t w = 0;
     for (size_t k = n_created; k-- > 0;) m.pt[w++] = created[k];      // last created = list head
-    for (size_t k = 0; k < n_exist; ++k) if (alive[k]) m.pt[w++] = existing[k];
+    for (size_t k = 0; k < n_exist; ++k) {
+        if (!alive[k]) continue;
+        if (w > slot[k]) hit(MB_MOVE_UP);
+        if (w < slot[k]) hit(MB_MOVE_DOWN);
+        if (similar[k]) hit(w == slot[k] ? MB_SIMILAR_INPLACE : MB_SIMILAR_MOVED);
+        m.pt[w++] = existing[k];
+    }
     m.num = uint32_t(w);
+    if (w == 4) hit(MB_FULL4);
+    if ((t >> MB_MOVE_UP & 1u) && (t >> MB_MOVE_DOWN & 1u)) hit(MB_MOVE_BOTH);
+    if (tr) *tr = t;
 }
 
 void World::narrowphase() {
+    if (trace_merge) merge_trace.assign(manifolds.size(), 0);
     parallel_for(threads, manifolds.size(), [&](size_t mi) {
         Manifold &m = manifolds[mi];
         const Body &A = bodies[m.a], &B = bodies[m.b];
@@ -422,7 +489,7 @@ void World::narrowphase() {
         }
         cresult res;
         detect_collision(A.sh, B.sh, A.pos, A.orn, A.bb, B.pos, B.orn, B.bb, res);
-        process_collision(m, res, A, B, dt);
+        process_collision(m, res, A, B, dt, trace_merge ? &merge_trace[mi] : nullptr);
     });
 }
 

@@ -55,6 +55,50 @@ struct Manifold {            // contact_manifold + state; pt[0] is the linked-li
     Point pt[4];
 };
 
+// Branches of process_collision (World::narrowphase), one bit each in World::merge_trace when trace_merge is on.  Test
+// infrastructure: tests/golden/make_merge.py samples cases until each branch is covered, and the merge tests assert that
+// coverage on the cases they run.  "Slot" is a point's position in the list when the step starts (the device's storage
+// slot), "index" its position once the removals of the first pass closed the gaps.
+enum merge_branch : uint32_t {
+    MB_SETTLED,             // persisted points present, every result point merged into one in the first pass
+    MB_EARLY_RETURN,        // no persisted point, empty result
+    MB_EMPTY_KEEP,          // empty result, a persisted point kept (distance updated)
+    MB_EMPTY_REMOVE,        // empty result, a persisted point removed
+    MB_NEAREST_A,           // merged into the result point nearest through pivot A
+    MB_NEAREST_B,           // ... through pivot B
+    MB_ROLL_A,              // merged through the rolling search on body A
+    MB_ROLL_B,              // ... on body B (pivotB, B's pose, the result's pivotA)
+    MB_ROLL_BOTH,           // both bodies rolling: B's search ran after A's found nothing
+    MB_TAKEN,               // the nearest result point was already merged: falls through to the removal test
+    MB_REMOVE_NORMAL,       // removed: separation along the normal
+    MB_REMOVE_TANGENT,      // removed: tangential drift only
+    MB_REMOVE_FIRST,        // removed slot 0 of 2+ points
+    MB_REMOVE_MIDDLE,       // removed a slot between the first and the last
+    MB_REMOVE_LAST,         // removed the last slot of 2+ points
+    MB_REMOVE_GAP,          // removed two slots with a kept one between them
+    MB_REMOVE_ALL4,         // removed all of 4 points
+    MB_KEPT,                // unmatched point kept, distance updated
+    MB_INS1_APPEND, MB_INS1_SIMILAR,
+    MB_INS2_APPEND, MB_INS2_SIMILAR, MB_INS2_REPLACE0, MB_INS2_REPLACE1, MB_INS2_NONE,
+    MB_INS3_NONE,           // in the triangle
+    MB_INS3_APPEND,
+    MB_INS3_COL1, MB_INS3_COL0, MB_INS3_COL2, MB_INS3_SHORTEST,     // collinear triple: replace index 1, 0, 2, shortest edge
+    MB_INS4_SIMILAR, MB_INS4_REPLACE0, MB_INS4_REPLACE1, MB_INS4_REPLACE2, MB_INS4_REPLACE3, MB_INS4_NONE,
+    MB_PIVOT_B,             // pivots B tried after pivots A found no place, and found one
+    MB_SIMILAR_INPLACE,     // SIMILAR onto a persisted point that stays in its slot
+    MB_SIMILAR_MOVED,       // SIMILAR onto a persisted point that changes slot (with its impulse)
+    MB_SIMILAR_CREATED,     // SIMILAR onto a point inserted this pass: created
+    MB_REPLACE_PERSISTED,   // REPLACE of a persisted point
+    MB_REPLACE_AFTER_GAP,   // ... that sat after a removed slot
+    MB_REPLACE_THEN_SIMILAR,// one index of the list written twice in one pass: REPLACE, then SIMILAR
+    MB_SIMILAR_THEN_REPLACE,//                                                     SIMILAR, then REPLACE
+    MB_FULL4,               // the rearranged list holds 4 points
+    MB_MOVE_UP,             // a persisted point moves to a later slot
+    MB_MOVE_DOWN,           // ... to an earlier slot
+    MB_MOVE_BOTH,           // both in one manifold
+    MB_COUNT
+};
+
 struct Hinge {               // constraints/hinge_constraint.hpp:22-93 without limits/springs/torque
     uint32_t a, b;
     vec3 pivot[2];
@@ -80,6 +124,8 @@ struct World {
     std::vector<double> isl_sleep_ts;                       // per previous label: island::sleep_timestamp, < 0 = unset
     void update_sleep();
     void wake_body(uint32_t i) { bodies[i].asleep = false; }
+    bool trace_merge = false;                               // record merge_trace in the next narrowphase
+    std::vector<uint64_t> merge_trace;                      // per manifold: bit b = merge_branch b was taken
     // Optional injected Gauss-Seidel order (see ora_api.cpp: ora_set_order).
     bool use_order = false;
     std::vector<uint32_t> hinge_order;
@@ -153,7 +199,7 @@ bool contact_solve_position(Point &cp, Body &A, Body &B, scalar &max_error);
 void hinge_solve_position(const Hinge &hc, Body &A, Body &B, scalar &max_error);   // hinge_constraint.cpp:180-213
 // the three decisions process_collision takes per persisted point (util/collision_util.cpp:233-280, :397-413), pinned
 // against the reference functions cut out of that unit at build time
-size_t find_nearest_contact(const Point &cp, const cresult &res);
+size_t find_nearest_contact(const Point &cp, const cresult &res, bool *via_B = nullptr);
 size_t find_nearest_contact_rolling(const cresult &res, vec3 cp_pivot, vec3 origin, quat orn, vec3 angvel, scalar dt);
 bool should_remove_point(const Point &cp, vec3 posA, quat ornA, vec3 posB, quat ornB);
 void solve_friction(FrictionPair &f, scalar normal_impulse, scalar inv_mA, const mat3 &inv_IA, scalar inv_mB, const mat3 &inv_IB,

@@ -18,6 +18,15 @@ STEPPER_SO = os.path.join(HERE, "_ref", "libedyn_stepper.so")
 SH_SPHERE, SH_CAPSULE, SH_BOX, SH_PLANE, SH_NONE = 0, 2, 3, 6, 255
 DYNAMIC, KINEMATIC, STATIC = 0, 1, 2
 PH_BROAD, PH_NARROW, PH_ISLANDS, PH_SOLVE = 1, 2, 4, 8
+# process_collision's branches in the order of merge_branch (ora_world.hpp): bit positions of OracleWorld.merge_trace()
+MERGE_BRANCHES = (
+    "settled", "early_return", "empty_keep", "empty_remove", "nearest_a", "nearest_b", "roll_a", "roll_b", "roll_both",
+    "taken", "remove_normal", "remove_tangent", "remove_first", "remove_middle", "remove_last", "remove_gap", "remove_all4",
+    "kept", "ins1_append", "ins1_similar", "ins2_append", "ins2_similar", "ins2_replace0", "ins2_replace1", "ins2_none",
+    "ins3_none", "ins3_append", "ins3_col1", "ins3_col0", "ins3_col2", "ins3_shortest", "ins4_similar", "ins4_replace0",
+    "ins4_replace1", "ins4_replace2", "ins4_replace3", "ins4_none", "pivot_b", "similar_inplace", "similar_moved",
+    "similar_created", "replace_persisted", "replace_after_gap", "replace_then_similar", "similar_then_replace", "full4",
+    "move_up", "move_down", "move_both")
 
 _f = np.float32
 _u = np.uint32
@@ -56,7 +65,7 @@ def lib():
         _lib.ora_create.restype = C.c_void_p
         _lib.ora_create.argtypes = [C.c_float, C.c_int, C.c_int, C.c_int]
         _lib.ora_solve_row.restype = C.c_float
-        for name in ("ora_num_bodies", "ora_num_manifolds"):
+        for name in ("ora_num_bodies", "ora_num_manifolds", "ora_get_merge_trace"):
             getattr(_lib, name).restype = C.c_uint32
     return _lib
 
@@ -384,6 +393,17 @@ class OracleWorld:
             u[:, :, 1] = _arr(lifetime, _u, (m, 4))
         self.l.ora_set_contacts(self.h, C.c_uint32(m), _ptr(pairs), _ptr(num), _ptr(pts), _ptr(u))
 
+    def set_merge_trace(self, on=True):
+        """Record, in every following narrowphase, which branches of process_collision each manifold took."""
+        self.l.ora_set_merge_trace(self.h, C.c_int(1 if on else 0))
+
+    def merge_trace(self):
+        """One uint64 per manifold from the last narrowphase: bit b = branch b of MERGE_BRANCHES was taken."""
+        m = int(self.l.ora_num_manifolds(self.h))
+        out = np.zeros(max(m, 1), np.uint64)
+        self.l.ora_get_merge_trace(self.h, _ptr(out))
+        return out[:m]
+
     def islands(self):
         lab = np.zeros(self.num_bodies, _u)
         self.l.ora_get_islands(self.h, _ptr(lab))
@@ -574,6 +594,31 @@ class RefWorld:
         lab = np.zeros(self.num_bodies, _u)
         self.l.refs_get_islands(self.h, _ptr(lab))
         return lab
+
+    def seed_manifolds(self, pairs, num, pts, att, lifetime):
+        """Manifolds with given points (layout of World.upload_contacts: pts (m, 4, 18), slot 0 = list head), made by the
+        reference's make_contact_manifold / create_contact_point and patched to the given values (refs_seed_manifolds)."""
+        pairs = _arr(pairs, _u, (-1, 2))
+        m = len(pairs)
+        u = np.zeros((m, 4, 2), _u)
+        u[:, :, 0], u[:, :, 1] = _arr(att, _u, (m, 4)), _arr(lifetime, _u, (m, 4))
+        num, pts = _arr(num, _u, (m,)), _arr(pts, _f, (m, 4, 18))
+        if self.l.refs_seed_manifolds(self.h, C.c_uint32(m), _ptr(pairs), _ptr(num), _ptr(pts), _ptr(u)):
+            raise RuntimeError("refs_seed_manifolds: bad body index or point count")
+        self.num_seeded = getattr(self, "num_seeded", 0) + m
+
+    def narrowphase(self):
+        """The reference's narrowphase::update(false) alone: contact distances, detect_collision, process_collision."""
+        self.l.refs_narrowphase(self.h)
+
+    def seeded(self):
+        """The seeded manifolds in seeding order: dict(num, pts (m, 4, 18), att, lifetime), as World.contacts()."""
+        m = getattr(self, "num_seeded", 0)
+        num, pts, u = np.zeros(max(m, 1), _u), np.zeros((max(m, 1), 4, 18), _f), np.zeros((max(m, 1), 4, 2), _u)
+        rc = self.l.refs_get_seeded(self.h, C.c_uint32(m), _ptr(num), _ptr(pts), _ptr(u))
+        if rc:
+            raise RuntimeError(f"refs_get_seeded: {rc}")
+        return dict(num=num[:m], pts=pts[:m], att=u[:m, :, 0].copy(), lifetime=u[:m, :, 1].copy())
 
     def solver_order(self, max_contacts=None):
         """(hinge indices, (n, 3) contact rows as body0, body1, point index) of the last step, in the reference's row order."""

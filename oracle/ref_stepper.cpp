@@ -6,6 +6,8 @@
 // The restitution solver's result depends on orders inside the entity graph at the moment solver::update starts, so
 // refs_step_begin / refs_step_end run stepper_sequential::step_simulation (stepper_sequential.cpp:121-147) in two halves;
 // that needs its three members, hence the access hack on this ONE header (object layout is unaffected).
+// refs_seed_manifolds / refs_narrowphase / refs_get_seeded run the reference's narrowphase alone on manifolds with given
+// points (tests/golden/make_merge.py).
 #define private public
 #include <edyn/simulation/stepper_sequential.hpp>
 #undef private
@@ -17,6 +19,8 @@
 #include <edyn/constraints/hinge_constraint.hpp>
 #include <edyn/collision/contact_manifold.hpp>
 #include <edyn/collision/contact_point.hpp>
+#include <edyn/collision/collision_result.hpp>
+#include <edyn/util/collision_util.hpp>
 #include <edyn/comp/position.hpp>
 #include <edyn/comp/orientation.hpp>
 #include <edyn/comp/linvel.hpp>
@@ -38,6 +42,7 @@
 #include <cstdint>
 #include <cstring>
 #include <memory>
+#include <optional>
 #include <vector>
 
 // Two entry points of the networking layer that the asynchronous stepper's translation units mention; the networking
@@ -59,6 +64,7 @@ namespace {
 struct World {
     entt::registry registry;
     std::vector<entt::entity> bodies, hinges;
+    std::vector<entt::entity> seeded;                       // manifolds made by refs_seed_manifolds, in argument order
     double time = 0.0, dt = 1.0 / 60;
     uint64_t steps = 0;
 };
@@ -261,6 +267,72 @@ REFS_API uint32_t refs_get_contacts(void *h, uint32_t capacity, uint32_t *pairs,
         ++n;
     }
     return n;
+}
+// ---- process_collision on given manifolds (tests/golden/make_merge.py).  Layout of b2d_upload_contacts (include/b2d.h):
+// per manifold 4 point slots, slot 0 = list head (newest); pt18 = pivotA(3) pivotB(3) normal(3) local_normal(3) distance
+// friction restitution normal_impulse friction_impulse[2]; pt_u2 = {normal_attachment, lifetime}.
+// Seeds manifolds with make_contact_manifold and their points with create_contact_point, last slot first so that slot 0
+// ends up at the head, then patches every persisted field to the given value.  No broadphase runs on these bodies.
+REFS_API int refs_seed_manifolds(void *h, uint32_t n, const uint32_t *pairs, const uint32_t *num, const float *pt18, const uint32_t *pt_u2) {
+    auto *w = static_cast<World *>(h);
+    auto &r = w->registry;
+    for (uint32_t k = 0; k < n; ++k) {
+        if (pairs[2 * k] >= w->bodies.size() || pairs[2 * k + 1] >= w->bodies.size() || num[k] > 4) return -1;
+        const auto me = edyn::make_contact_manifold(r, w->bodies[pairs[2 * k]], w->bodies[pairs[2 * k + 1]]);
+        w->seeded.push_back(me);
+        for (uint32_t s = num[k]; s-- > 0;) {
+            const float *f = pt18 + ((size_t)k * 4 + s) * 18;
+            const uint32_t *u = pt_u2 + ((size_t)k * 4 + s) * 2;
+            auto &manifold = r.get<edyn::contact_manifold>(me);
+            auto &state = r.get<edyn::contact_manifold_state>(me);
+            edyn::collision_result::collision_point rp;
+            rp.pivotA = v3(f); rp.pivotB = v3(f + 3); rp.normal = v3(f + 6); rp.distance = f[12];
+            rp.normal_attachment = static_cast<edyn::contact_normal_attachment>(u[0]);
+            const auto ce = edyn::create_contact_point(r, me, manifold, state, rp, std::nullopt);
+            r.get<edyn::contact_point>(ce).lifetime = u[1];
+            auto &geom = r.get<edyn::contact_point_geometry>(ce);
+            geom.local_normal = v3(f + 9); geom.normal_attachment = rp.normal_attachment; geom.distance = f[12];
+            auto &mat = r.get<edyn::contact_point_material>(ce);
+            mat.friction = f[13]; mat.restitution = f[14];
+            auto &imp = r.get<edyn::contact_point_impulse>(ce);
+            imp.normal_impulse = f[15]; imp.friction_impulse = {f[16], f[17]};
+        }
+    }
+    return 0;
+}
+// the reference's own narrowphase, as refs_step_begin calls it: update_contact_distances, then detect_collision and
+// process_collision with the sequential create / destroy functors on every awake manifold
+REFS_API void refs_narrowphase(void *h) {
+    auto *w = static_cast<World *>(h);
+    w->registry.ctx().get<edyn::narrowphase>().update(false);
+}
+// the seeded manifolds, in seeding order, in the layout of refs_seed_manifolds (slots past num are zero)
+REFS_API int refs_get_seeded(void *h, uint32_t n, uint32_t *num, float *pt18, uint32_t *pt_u2) {
+    auto *w = static_cast<World *>(h);
+    auto &r = w->registry;
+    if (n != w->seeded.size()) return -1;
+    std::memset(pt18, 0, (size_t)n * 4 * 18 * sizeof(float)); std::memset(pt_u2, 0, (size_t)n * 4 * 2 * sizeof(uint32_t));
+    for (uint32_t k = 0; k < n; ++k) {
+        const auto &state = r.get<edyn::contact_manifold_state>(w->seeded[k]);
+        num[k] = state.num_points;
+        uint32_t s = 0;
+        for (auto ce = state.contact_entity; ce != entt::null; ce = r.get<edyn::contact_point_list>(ce).next, ++s) {
+            if (s >= 4) return -2;
+            const auto &cp = r.get<edyn::contact_point>(ce);
+            const auto &geom = r.get<edyn::contact_point_geometry>(ce);
+            const auto &mat = r.get<edyn::contact_point_material>(ce);
+            const auto &imp = r.get<edyn::contact_point_impulse>(ce);
+            float *o = pt18 + ((size_t)k * 4 + s) * 18;
+            const edyn::vector3 vs[4] = {cp.pivotA, cp.pivotB, cp.normal, geom.local_normal};
+            for (int j = 0; j < 4; ++j) { o[3 * j] = vs[j].x; o[3 * j + 1] = vs[j].y; o[3 * j + 2] = vs[j].z; }
+            o[12] = geom.distance; o[13] = mat.friction; o[14] = mat.restitution;
+            o[15] = imp.normal_impulse; o[16] = imp.friction_impulse[0]; o[17] = imp.friction_impulse[1];
+            pt_u2[((size_t)k * 4 + s) * 2] = uint32_t(geom.normal_attachment);
+            pt_u2[((size_t)k * 4 + s) * 2 + 1] = cp.lifetime;
+        }
+        if (s != state.num_points) return -3;
+    }
+    return 0;
 }
 // ---- what user code does between steps (plain registry / public API calls)
 REFS_API void refs_destroy_body(void *h, uint32_t body) {                      // registry.destroy(entity)
