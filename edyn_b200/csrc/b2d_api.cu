@@ -157,6 +157,7 @@ b2d_world *b2d_create(const b2d_config *cfg) {
     ok = ok && dalloc(w, d.grav, NB) && dalloc(w, d.shp, NB) && dalloc(w, d.bbmin, NB) && dalloc(w, d.bbmax, NB);
     ok = ok && dalloc(w, d.flags, NB) && dalloc(w, d.mat, NB) && dalloc(w, d.group, NB) && dalloc(w, d.fmask, NB);
     ok = ok && dalloc(w, d.cellkey, NB) && dalloc(w, d.cellkey_s, NB) && dalloc(w, d.cellbody, NB) && dalloc(w, d.cellbody_s, NB) && dalloc(w, d.brank, NB);
+    ok = ok && dalloc(w, d.bprec_min, NB) && dalloc(w, d.bprec_max, NB) && dalloc(w, d.cell_box, 6);
     d.chash_size = pow2_at_least(2ull * NB);
     ok = ok && dalloc(w, d.chash_key, d.chash_size, 0xFF) && dalloc(w, d.chash_val, d.chash_size);
     ok = ok && dalloc(w, d.large_list, NB) && dalloc(w, d.newcount, NB) && dalloc(w, d.newoff, NB) && dalloc(w, d.newpairs, NM);
@@ -551,7 +552,8 @@ static int enqueue_broadphase(b2d_world *w) {
     CK(cub::DeviceScan::ExclusiveSum(w->cub_tmp, t, d.free_flag, d.free_rank, (int)d.NM, s)); ++w->launches;
     LAUNCH(k_bp_free_list, d.NM, 256, d);
     if (d.nbodies) {
-        LAUNCH(k_bp_cells, d.nbodies, 256, d, d.cellkey, d.cellbody);
+        CK(cudaMemsetAsync(d.cell_box, 0xFF, 6 * sizeof(uint32_t), s));
+        LAUNCH(k_bp_cells, d.nbodies, 256, d, d.cellkey, d.cellbody, d.cell_box);
         t = w->cub_tmp_bytes;
         CK(cub::DeviceRadixSort::SortPairs(w->cub_tmp, t, d.cellkey, d.cellkey_s, d.cellbody, d.cellbody_s, (int)d.nbodies, 0, w->cell_key_bits, s)); w->launches += 4;
         LAUNCH(k_bp_cell_starts, d.nbodies, 256, d);
@@ -1224,7 +1226,7 @@ static int ray_index(b2d_world *w) {
     if (w->ray_epoch == w->state_epoch) return B2D_OK;
     LAUNCH(k_ray_reset, 1, 32, x);
     if (d.nbodies) {
-        LAUNCH(k_bp_cells, d.nbodies, 256, d, x.key, x.body);
+        LAUNCH(k_bp_cells, d.nbodies, 256, d, x.key, x.body, (uint32_t *)nullptr);
         LAUNCH(k_ray_classify, d.nbodies, 256, d, x);
         size_t t = w->cub_tmp_bytes;
         CK(cub::DeviceRadixSort::SortPairs(w->cub_tmp, t, x.key, x.key_s, x.body, x.body_s, (int)d.nbodies, 0, w->cell_key_bits, s)); w->launches += 4;

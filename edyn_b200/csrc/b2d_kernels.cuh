@@ -173,28 +173,62 @@ __global__ void k_bp_free_list(Dev d) {
 // passes are paid per key byte, so the host sizes the fields to the extent the world had when the step was captured).
 // Cells beyond the range share the boundary key, which only makes the candidate lists there longer: every pair still
 // goes through the exact AABB tests.  All-ones is reserved for "no cell".
-B2D_D unsigned long long cell_key_of(const Dev &d, int cx, int cy, int cz) {
-    const unsigned long long x = (unsigned long long)min(max(cx - d.cell_org[0], 0), (1 << d.cell_bits[0]) - 2);
-    const unsigned long long y = (unsigned long long)min(max(cy - d.cell_org[1], 0), (1 << d.cell_bits[1]) - 1);
-    const unsigned long long z = (unsigned long long)min(max(cz - d.cell_org[2], 0), (1 << d.cell_bits[2]) - 1);
-    return (x << (d.cell_bits[1] + d.cell_bits[2])) | (y << d.cell_bits[2]) | z;
+struct CellFields { uint32_t x, y, z; };
+B2D_D CellFields cell_fields(const Dev &d, int cx, int cy, int cz) {
+    return CellFields{(uint32_t)min(max(cx - d.cell_org[0], 0), (1 << d.cell_bits[0]) - 2),
+                      (uint32_t)min(max(cy - d.cell_org[1], 0), (1 << d.cell_bits[1]) - 1),
+                      (uint32_t)min(max(cz - d.cell_org[2], 0), (1 << d.cell_bits[2]) - 1)};
 }
-B2D_D void cell_of(const Dev &d, uint32_t i, int &cx, int &cy, int &cz) {
-    float4 a = d.bbmin[i], b = d.bbmax[i];
+B2D_D unsigned long long cell_key(const Dev &d, CellFields f) {
+    return ((unsigned long long)f.x << (d.cell_bits[1] + d.cell_bits[2])) | ((unsigned long long)f.y << d.cell_bits[2]) | f.z;
+}
+B2D_D unsigned long long cell_key_of(const Dev &d, int cx, int cy, int cz) { return cell_key(d, cell_fields(d, cx, cy, cz)); }
+// The box of key fields occupied this step (k_bp_cells): a cell outside it is empty, so its hash probe is skipped.
+struct CellBox { uint32_t lo[3], hi[3]; };
+B2D_D CellBox load_cell_box(const Dev &d) {
+    CellBox b;
+    #pragma unroll
+    for (int k = 0; k < 3; ++k) { b.lo[k] = d.cell_box[k]; b.hi[k] = ~d.cell_box[3 + k]; }
+    return b;
+}
+B2D_D bool in_cell_box(const CellBox &b, CellFields f) {
+    return f.x >= b.lo[0] && f.x <= b.hi[0] && f.y >= b.lo[1] && f.y <= b.hi[1] && f.z >= b.lo[2] && f.z <= b.hi[2];
+}
+B2D_D void cell_of(const Dev &d, float4 a, float4 b, int &cx, int &cy, int &cz) {
     cx = (int)floorf((a.x + b.x) * 0.5f * d.inv_cell);
     cy = (int)floorf((a.y + b.y) * 0.5f * d.inv_cell);
     cz = (int)floorf((a.z + b.z) * 0.5f * d.inv_cell);
 }
+B2D_D void cell_of(const Dev &d, uint32_t i, int &cx, int &cy, int &cz) { cell_of(d, d.bbmin[i], d.bbmax[i], cx, cy, cz); }
 
 // Cell key per body.  Shapeless and "large" bodies get the all-ones key and sort to the end.  The broadphase writes
-// d.cellkey / d.cellbody; the raycast index (k_ray_*) its own arrays.
-__global__ void k_bp_cells(Dev d, unsigned long long *cellkey, uint32_t *cellbody) {
+// d.cellkey / d.cellbody and the occupied box of key fields (box: min field, then min of the complemented field, both
+// preset to all-ones); the raycast index (k_ray_*) its own arrays and no box.
+__global__ void k_bp_cells(Dev d, unsigned long long *cellkey, uint32_t *cellbody, uint32_t *box) {
+    uint32_t m[6] = {~0u, ~0u, ~0u, ~0u, ~0u, ~0u};
     GRID_STRIDE(i, d.nbodies) {
         uint32_t f = d.flags[i];
         unsigned long long key = EMPTY_KEY;
-        if (shape_of(f) != SH_NONE && !(f & F_LARGE)) { int cx, cy, cz; cell_of(d, i, cx, cy, cz); key = cell_key_of(d, cx, cy, cz); }
+        if (shape_of(f) != SH_NONE && !(f & F_LARGE)) {
+            int cx, cy, cz; cell_of(d, i, cx, cy, cz);
+            const CellFields c = cell_fields(d, cx, cy, cz);
+            key = cell_key(d, c);
+            m[0] = min(m[0], c.x); m[1] = min(m[1], c.y); m[2] = min(m[2], c.z);
+            m[3] = min(m[3], ~c.x); m[4] = min(m[4], ~c.y); m[5] = min(m[5], ~c.z);
+        }
         cellkey[i] = key; cellbody[i] = i;
     }
+    if (!box) return;
+    __shared__ uint32_t sm[6];
+    if (threadIdx.x < 6) sm[threadIdx.x] = ~0u;
+    __syncthreads();
+    #pragma unroll
+    for (int k = 0; k < 6; ++k) {
+        m[k] = __reduce_min_sync(0xffffffffu, m[k]);
+        if ((threadIdx.x & 31) == 0) atomicMin(&sm[k], m[k]);
+    }
+    __syncthreads();
+    if (threadIdx.x < 6 && sm[threadIdx.x] != ~0u) atomicMin(&box[threadIdx.x], sm[threadIdx.x]);
 }
 // Cells occupied by the bodies that go into the grid (host: sizes the key fields, b2d_api.cu measure_cells)
 __global__ void k_cell_extent(Dev d, int *out6) {
@@ -223,13 +257,18 @@ B2D_D uint32_t key_body(const Dev &d, uint2 pr) {
 }
 // spatial part of a dataflow manifold's sort key (k_color_keys): the key body's rank in the cell order, 14 bits
 B2D_D uint32_t df_spatial(const Dev &d, uint32_t rank) { return (uint32_t)(((unsigned long long)rank << KEY_DF_SPATIAL_BITS) / d.nbodies); }
-// First sorted index of every occupied cell -> hash table.  A body that is not in an island tile and whose spatial
-// rank moved would change a dataflow sort key: the island rebuild has to run.
+// First sorted index of every occupied cell -> hash table, and every body's candidate record in the sorted order (what
+// bp_candidate reads about it), so the neighbourhood search walks records instead of gathering by body id.  A body that
+// is not in an island tile and whose spatial rank moved would change a dataflow sort key: the island rebuild has to run.
 __global__ void k_bp_cell_starts(Dev d) {
     GRID_STRIDE(i, d.nbodies) {
+        // the gathers first: they are independent of each other and of the hash insert's atomics
+        const uint32_t b = d.cellbody_s[i];
+        const float4 mn = d.bbmin[b], mx = d.bbmax[b];
+        d.bprec_min[i] = make_float4(mn.x, mn.y, mn.z, __uint_as_float(b));
+        d.bprec_max[i] = make_float4(mx.x, mx.y, mx.z, __uint_as_float(d.flags[b]));
         unsigned long long k = d.cellkey_s[i];
         if (k != EMPTY_KEY && (i == 0 || d.cellkey_s[i - 1] != k)) hash_insert(d.chash_key, d.chash_val, d.chash_size, k, i);
-        const uint32_t b = d.cellbody_s[i];
         if (df_spatial(d, d.brank[b]) != df_spatial(d, i) && d.btile[b] == TILE_NONE) d.cnt->graph_changed = 1u;
         d.brank[b] = i;
     }
@@ -252,14 +291,14 @@ B2D_D bool should_collide(const Dev &d, uint32_t a, uint32_t fa, uint32_t b, uin
 // (its AABB inflated by 0.02) hits the other's AABB, whichever is iterated first (broadphase.cpp:183-194,
 // :136-155).  Each unordered pair is evaluated by exactly one thread: the one of the higher-id procedural
 // body (views are assumed to iterate newest-first, SURVEY.md appendix A.11), which therefore becomes body[0].
-B2D_D void bp_candidate(const Dev &d, uint32_t A, uint32_t fA, const box3 &bbA, const box3 &qA, uint32_t j,
-                        uint32_t &count, uint2 *out) {
+// (j, fj, bbj) are the candidate's id, flags and AABB, from its cell-ordered record (bp_candidate_rec) or gathered by
+// id (bp_candidate_id).
+B2D_D void bp_candidate(const Dev &d, uint32_t A, uint32_t fA, const box3 &bbA, const box3 &qA, uint32_t j, uint32_t fj,
+                        const box3 &bbj, uint32_t &count, uint2 *out) {
     if (j == A) return;
-    uint32_t fj = d.flags[j];
     if (shape_of(fj) == SH_NONE) return;
     bool pj = is_dynamic(fj);
     if (pj && j > A) return;
-    box3 bbj = body_box(d, j);
     uint32_t first = A, second = j;
     if (pj) {
         bool t1 = intersect(qA, bbj);
@@ -274,17 +313,53 @@ B2D_D void bp_candidate(const Dev &d, uint32_t A, uint32_t fA, const box3 &bbA, 
     if (out) out[count] = make_uint2(first, second);
     ++count;
 }
+B2D_D void bp_candidate_id(const Dev &d, uint32_t A, uint32_t fA, const box3 &bbA, const box3 &qA, uint32_t j,
+                           uint32_t &count, uint2 *out) {
+    bp_candidate(d, A, fA, bbA, qA, j, d.flags[j], body_box(d, j), count, out);
+}
+B2D_D box3 rec_box(float4 mn, float4 mx) { box3 b; b.mn = mk3(mn); b.mx = mk3(mx); return b; }
+B2D_D void bp_candidate_rec(const Dev &d, uint32_t A, uint32_t fA, const box3 &bbA, const box3 &qA, uint32_t k,
+                            uint32_t &count, uint2 *out) {
+    const float4 mn = d.bprec_min[k], mx = d.bprec_max[k];
+    bp_candidate(d, A, fA, bbA, qA, __float_as_uint(mn.w), __float_as_uint(mx.w), rec_box(mn, mx), count, out);
+}
 
-#ifndef B2D_BP_CELL_ORDER
-#define B2D_BP_CELL_ORDER 1
-#endif
+// One column of the 27-cell neighbourhood: the cells (x, y, cz - 1 .. cz + 1).  z is the key's low field, so cells with
+// consecutive keys are one run of the sorted records, and one walk from the run's first occupied cell visits them in the
+// order of a probe and a walk per cell.  Where cell_key_of clamps z (outside the extent measured at capture), two or
+// three offsets share a key; each offset walks that cell again, as a probe and a walk per offset did, so a pair there is
+// emitted once per offset.
+struct BpColumn { unsigned long long key[3]; uint32_t start[3]; bool occ[3]; };
+B2D_D BpColumn bp_column_find(const Dev &d, const CellBox &box, int x, int y, int cz) {
+    BpColumn c;
+    #pragma unroll
+    for (int z = 0; z < 3; ++z) {
+        const CellFields f = cell_fields(d, x, y, cz + z - 1);
+        c.key[z] = cell_key(d, f);
+        c.occ[z] = in_cell_box(box, f) && hash_find(d.chash_key, d.chash_val, d.chash_size, c.key[z], c.start[z]);
+    }
+    return c;
+}
+B2D_D void bp_column_walk(const Dev &d, const BpColumn &c, uint32_t A, uint32_t fA, const box3 &bbA, const box3 &qA,
+                          uint32_t &count, uint2 *out) {
+    bool found = false; uint32_t k = 0;
+    #pragma unroll
+    for (int z = 0; z < 3; ++z) {
+        if (!found && c.occ[z]) { found = true; k = c.start[z]; }
+        if (z == 2 || c.key[z + 1] != c.key[z] + 1) {             // the run ends at cell z
+            if (found) for (; k < d.nbodies && d.cellkey_s[k] <= c.key[z]; ++k) bp_candidate_rec(d, A, fA, bbA, qA, k, count, out);
+            found = false;
+        }
+    }
+}
+
 template<bool FILL>
 __global__ void k_bp_pairs(Dev d) {
     GRID_STRIDE(t, d.nbodies) {
         // threads walk the bodies in cell order: a warp's queries hit the same cells and candidate records (output
         // slots are still indexed by body id, so the pair order does not change)
-        const uint32_t A = B2D_BP_CELL_ORDER ? d.cellbody_s[t] : t;
-        uint32_t fA = d.flags[A];
+        const float4 rmn = d.bprec_min[t], rmx = d.bprec_max[t];
+        const uint32_t A = __float_as_uint(rmn.w), fA = __float_as_uint(rmx.w);
         uint32_t count = 0;
         uint2 *out = nullptr;
         if (FILL) {
@@ -295,36 +370,33 @@ __global__ void k_bp_pairs(Dev d) {
             out = d.newpairs + d.newoff[A];
         }
         if (is_dynamic(fA) && shape_of(fA) != SH_NONE) {
-            box3 bbA = body_box(d, A);
-            box3 qA = inset(bbA, BP_OFFSET);
+            const box3 bbA = rec_box(rmn, rmx);
+            const box3 qA = inset(bbA, BP_OFFSET);
             if (!(fA & F_LARGE)) {
-                int cx, cy, cz; cell_of(d, A, cx, cy, cz);
-                for (int dx = -1; dx <= 1; ++dx) for (int dy = -1; dy <= 1; ++dy) for (int dz = -1; dz <= 1; ++dz) {
-                    unsigned long long key = cell_key_of(d, cx + dx, cy + dy, cz + dz);
-                    uint32_t start;
-                    if (!hash_find(d.chash_key, d.chash_val, d.chash_size, key, start)) continue;
-                    for (uint32_t k = start; k < d.nbodies && d.cellkey_s[k] == key; ++k)
-                        bp_candidate(d, A, fA, bbA, qA, d.cellbody_s[k], count, out);
-                }
+                int cx, cy, cz; cell_of(d, rmn, rmx, cx, cy, cz);
+                const CellBox box = load_cell_box(d);
+                for (int dx = -1; dx <= 1; ++dx) for (int dy = -1; dy <= 1; ++dy)
+                    bp_column_walk(d, bp_column_find(d, box, cx + dx, cy + dy, cz), A, fA, bbA, qA, count, out);
             } else {
-                for (uint32_t j = 0; j < d.nbodies; ++j) if (!(d.flags[j] & F_LARGE)) bp_candidate(d, A, fA, bbA, qA, j, count, out);
+                for (uint32_t j = 0; j < d.nbodies; ++j) if (!(d.flags[j] & F_LARGE)) bp_candidate_id(d, A, fA, bbA, qA, j, count, out);
             }
-            for (uint32_t k = 0; k < d.nlarge; ++k) bp_candidate(d, A, fA, bbA, qA, d.large_list[k], count, out);
+            for (uint32_t k = 0; k < d.nlarge; ++k) bp_candidate_id(d, A, fA, bbA, qA, d.large_list[k], count, out);
         }
         if (!FILL) d.newcount[A] = count;
     }
 }
 // The same search with one WARP per query body: lane c < 27 takes cell c of the neighbourhood (in the loop order of
-// the thread-per-body kernel), lane 27 the brute-force list, and a warp prefix sum of the lane counts puts the pairs in
-// exactly the order the serial walk produces.  27 hash probes and cell walks in flight per body instead of one after
-// the other: the search is latency-bound at small body counts (100 us for 4 096 bodies with a thread per body).
+// the thread-per-body kernel: its column walks visit the same cells in the same order), lane 27 the large list; a large
+// query body splits the brute-force list over lanes 0..26.  A warp prefix sum of the lane counts puts the pairs in
+// exactly the order the serial walk produces.  27 probes and cell walks in flight per body: the search is latency-bound
+// at small body counts, where a lane per column (three cells walked one after the other) was slower (DESIGN.md §2).
 template<bool FILL>
 __global__ void k_bp_pairs_warp(Dev d) {
     const uint32_t lane = threadIdx.x & 31u;
     const uint32_t wid = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
     for (uint32_t t = wid; t < d.nbodies; t += nw) {
-        const uint32_t A = d.cellbody_s[t];
-        const uint32_t fA = d.flags[A];
+        const float4 rmn = d.bprec_min[t], rmx = d.bprec_max[t];
+        const uint32_t A = __float_as_uint(rmn.w), fA = __float_as_uint(rmx.w);
         uint2 *out = nullptr;
         if (FILL) {
             if (d.newcount[A] == 0) continue;
@@ -333,15 +405,16 @@ __global__ void k_bp_pairs_warp(Dev d) {
         }
         uint32_t total = 0;
         if (is_dynamic(fA) && shape_of(fA) != SH_NONE) {
-            const box3 bbA = body_box(d, A);
+            const box3 bbA = rec_box(rmn, rmx);
             const box3 qA = inset(bbA, BP_OFFSET);
             // this lane's share of the candidates, walked once to count and (FILL) once more to write
             uint32_t start = 0, end = 0; unsigned long long key = EMPTY_KEY; int mode = 0;      // 0 nothing, 1 one cell, 2 a range of body ids, 3 the large list
             if (!(fA & F_LARGE)) {
                 if (lane < 27u) {
-                    int cx, cy, cz; cell_of(d, A, cx, cy, cz);
-                    key = cell_key_of(d, cx + (int)(lane / 9u) - 1, cy + (int)((lane / 3u) % 3u) - 1, cz + (int)(lane % 3u) - 1);
-                    if (hash_find(d.chash_key, d.chash_val, d.chash_size, key, start)) mode = 1;
+                    int cx, cy, cz; cell_of(d, rmn, rmx, cx, cy, cz);
+                    const CellFields f = cell_fields(d, cx + (int)(lane / 9u) - 1, cy + (int)((lane / 3u) % 3u) - 1, cz + (int)(lane % 3u) - 1);
+                    key = cell_key(d, f);
+                    if (in_cell_box(load_cell_box(d), f) && hash_find(d.chash_key, d.chash_val, d.chash_size, key, start)) mode = 1;
                 }
             } else if (lane < 27u) {
                 const uint32_t chunk = (d.nbodies + 26u) / 27u;
@@ -350,9 +423,9 @@ __global__ void k_bp_pairs_warp(Dev d) {
             if (lane == 27u) mode = 3;
             auto walk = [&](uint2 *o) {
                 uint32_t c = 0;
-                if (mode == 1) { for (uint32_t k = start; k < d.nbodies && d.cellkey_s[k] == key; ++k) bp_candidate(d, A, fA, bbA, qA, d.cellbody_s[k], c, o); }
-                else if (mode == 2) { for (uint32_t j = start; j < end; ++j) if (!(d.flags[j] & F_LARGE)) bp_candidate(d, A, fA, bbA, qA, j, c, o); }
-                else if (mode == 3) { for (uint32_t k = 0; k < d.nlarge; ++k) bp_candidate(d, A, fA, bbA, qA, d.large_list[k], c, o); }
+                if (mode == 1) { for (uint32_t k = start; k < d.nbodies && d.cellkey_s[k] == key; ++k) bp_candidate_rec(d, A, fA, bbA, qA, k, c, o); }
+                else if (mode == 2) { for (uint32_t j = start; j < end; ++j) if (!(d.flags[j] & F_LARGE)) bp_candidate_id(d, A, fA, bbA, qA, j, c, o); }
+                else if (mode == 3) { for (uint32_t k = 0; k < d.nlarge; ++k) bp_candidate_id(d, A, fA, bbA, qA, d.large_list[k], c, o); }
                 return c;
             };
             const uint32_t mine = walk(nullptr);

@@ -111,6 +111,8 @@ struct Dev {
     unsigned long long *cellkey, *cellkey_s;
     uint32_t *cellbody, *cellbody_s;
     uint32_t *brank;                     // position of every body in the sorted cell order (spatial rank)
+    float4 *bprec_min, *bprec_max;       // per sorted index: the body's AABB min | id and max | flags (candidate records)
+    uint32_t *cell_box;                  // occupied key fields this step: min x, y, z, then min of ~x, ~y, ~z (k_bp_cells)
     // ---- island tiles
     uint32_t max_tiles;
     uint32_t *isl_nb, *isl_nm, *isl_nh;  // per island root: dynamic bodies, manifolds with points (| ISL_MULTIPOINT), joints
