@@ -172,12 +172,15 @@ __global__ void k_bp_free_list(Dev d) {
 // Cell key: the three cell coordinates relative to d.cell_org, packed into d.cell_bits[0..2] bits each (radix sort
 // passes are paid per key byte, so the host sizes the fields to the extent the world had when the step was captured).
 // Cells beyond the range share the boundary key, which only makes the candidate lists there longer: every pair still
-// goes through the exact AABB tests.  All-ones is reserved for "no cell".
+// goes through the exact AABB tests.  Neighbour offsets that clamp to the same field are the same cells: clamping is
+// monotone, so they are adjacent, and the search skips an offset whose field repeats the previous offset's on some axis
+// (each cell is walked once per query body).  All-ones is reserved for "no cell", so x stops one short of its field's maximum.
 struct CellFields { uint32_t x, y, z; };
+B2D_D uint32_t cell_field(const Dev &d, int k, int c) {
+    return (uint32_t)min(max(c - d.cell_org[k], 0), (1 << d.cell_bits[k]) - (k == 0 ? 2 : 1));
+}
 B2D_D CellFields cell_fields(const Dev &d, int cx, int cy, int cz) {
-    return CellFields{(uint32_t)min(max(cx - d.cell_org[0], 0), (1 << d.cell_bits[0]) - 2),
-                      (uint32_t)min(max(cy - d.cell_org[1], 0), (1 << d.cell_bits[1]) - 1),
-                      (uint32_t)min(max(cz - d.cell_org[2], 0), (1 << d.cell_bits[2]) - 1)};
+    return CellFields{cell_field(d, 0, cx), cell_field(d, 1, cy), cell_field(d, 2, cz)};
 }
 B2D_D unsigned long long cell_key(const Dev &d, CellFields f) {
     return ((unsigned long long)f.x << (d.cell_bits[1] + d.cell_bits[2])) | ((unsigned long long)f.y << d.cell_bits[2]) | f.z;
@@ -327,8 +330,7 @@ B2D_D void bp_candidate_rec(const Dev &d, uint32_t A, uint32_t fA, const box3 &b
 // One column of the 27-cell neighbourhood: the cells (x, y, cz - 1 .. cz + 1).  z is the key's low field, so cells with
 // consecutive keys are one run of the sorted records, and one walk from the run's first occupied cell visits them in the
 // order of a probe and a walk per cell.  Where cell_key_of clamps z (outside the extent measured at capture), two or
-// three offsets share a key; each offset walks that cell again, as a probe and a walk per offset did, so a pair there is
-// emitted once per offset.
+// three offsets share a key; only the first of them is probed, so the cell is walked once and each pair found once.
 struct BpColumn { unsigned long long key[3]; uint32_t start[3]; bool occ[3]; };
 B2D_D BpColumn bp_column_find(const Dev &d, const CellBox &box, int x, int y, int cz) {
     BpColumn c;
@@ -336,7 +338,7 @@ B2D_D BpColumn bp_column_find(const Dev &d, const CellBox &box, int x, int y, in
     for (int z = 0; z < 3; ++z) {
         const CellFields f = cell_fields(d, x, y, cz + z - 1);
         c.key[z] = cell_key(d, f);
-        c.occ[z] = in_cell_box(box, f) && hash_find(d.chash_key, d.chash_val, d.chash_size, c.key[z], c.start[z]);
+        c.occ[z] = (z == 0 || c.key[z] != c.key[z - 1]) && in_cell_box(box, f) && hash_find(d.chash_key, d.chash_val, d.chash_size, c.key[z], c.start[z]);
     }
     return c;
 }
@@ -375,8 +377,13 @@ __global__ void k_bp_pairs(Dev d) {
             if (!(fA & F_LARGE)) {
                 int cx, cy, cz; cell_of(d, rmn, rmx, cx, cy, cz);
                 const CellBox box = load_cell_box(d);
-                for (int dx = -1; dx <= 1; ++dx) for (int dy = -1; dy <= 1; ++dy)
-                    bp_column_walk(d, bp_column_find(d, box, cx + dx, cy + dy, cz), A, fA, bbA, qA, count, out);
+                for (int dx = -1; dx <= 1; ++dx) {
+                    if (dx > -1 && cell_field(d, 0, cx + dx) == cell_field(d, 0, cx + dx - 1)) continue;      // clamped: same cells
+                    for (int dy = -1; dy <= 1; ++dy) {
+                        if (dy > -1 && cell_field(d, 1, cy + dy) == cell_field(d, 1, cy + dy - 1)) continue;
+                        bp_column_walk(d, bp_column_find(d, box, cx + dx, cy + dy, cz), A, fA, bbA, qA, count, out);
+                    }
+                }
             } else {
                 for (uint32_t j = 0; j < d.nbodies; ++j) if (!(d.flags[j] & F_LARGE)) bp_candidate_id(d, A, fA, bbA, qA, j, count, out);
             }
@@ -386,12 +393,14 @@ __global__ void k_bp_pairs(Dev d) {
     }
 }
 // The same search with one WARP per query body: lane c < 27 takes cell c of the neighbourhood (in the loop order of
-// the thread-per-body kernel: its column walks visit the same cells in the same order), lane 27 the large list; a large
+// the thread-per-body kernel: its column walks visit the same cells in the same order; a lane whose cell repeats an
+// earlier lane's clamped cell stays idle), lane 27 the large list; a large
 // query body splits the brute-force list over lanes 0..26.  A warp prefix sum of the lane counts puts the pairs in
 // exactly the order the serial walk produces.  27 probes and cell walks in flight per body: the search is latency-bound
 // at small body counts, where a lane per column (three cells walked one after the other) was slower (DESIGN.md §2).
 template<bool FILL>
-__global__ void k_bp_pairs_warp(Dev d) {
+// (launch bounds: the repeat test below costs registers; bounded, both passes keep at least the residency they had without it)
+__global__ void __launch_bounds__(256, FILL ? 5 : 8) k_bp_pairs_warp(Dev d) {
     const uint32_t lane = threadIdx.x & 31u;
     const uint32_t wid = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
     for (uint32_t t = wid; t < d.nbodies; t += nw) {
@@ -412,9 +421,13 @@ __global__ void k_bp_pairs_warp(Dev d) {
             if (!(fA & F_LARGE)) {
                 if (lane < 27u) {
                     int cx, cy, cz; cell_of(d, rmn, rmx, cx, cy, cz);
-                    const CellFields f = cell_fields(d, cx + (int)(lane / 9u) - 1, cy + (int)((lane / 3u) % 3u) - 1, cz + (int)(lane % 3u) - 1);
+                    const int ox = (int)(lane / 9u), oy = (int)((lane / 3u) % 3u), oz = (int)(lane % 3u);
+                    const CellFields f = cell_fields(d, cx + ox - 1, cy + oy - 1, cz + oz - 1);
                     key = cell_key(d, f);
-                    if (in_cell_box(load_cell_box(d), f) && hash_find(d.chash_key, d.chash_val, d.chash_size, key, start)) mode = 1;
+                    // a lane whose field repeats the previous offset's on some axis has the same cell as an earlier lane
+                    const bool repeat = (ox && f.x == cell_field(d, 0, cx + ox - 2)) || (oy && f.y == cell_field(d, 1, cy + oy - 2)) ||
+                                        (oz && f.z == cell_field(d, 2, cz + oz - 2));
+                    if (!repeat && in_cell_box(load_cell_box(d), f) && hash_find(d.chash_key, d.chash_val, d.chash_size, key, start)) mode = 1;
                 }
             } else if (lane < 27u) {
                 const uint32_t chunk = (d.nbodies + 26u) / 27u;

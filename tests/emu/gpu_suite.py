@@ -43,7 +43,7 @@ def main():
     Z.load = load
     files = [os.path.join(ROOT, "tests", f) for f in ("test_gpu_parity.py", "test_gpu_dist.py", "test_gpu_handover.py", "test_zz_gpu_stepper_b2d.py",
                                                       "test_gpu_tile_edges.py", "test_gpu_random_lockstep.py", "test_gpu_large_bodies.py",
-                                                      "test_gpu_merge.py", "test_gpu_point_transitions.py")]
+                                                      "test_gpu_merge.py", "test_gpu_point_transitions.py", "test_gpu_broadphase_edges.py")]
     return pytest.main(["-q", "-m", "gpu", "-k", SELECT, "-p", "no:cacheprovider"] + files + sys.argv[1:])
 
 

@@ -106,6 +106,9 @@ inline unsigned __match_any_sync(unsigned m, unsigned v) { return unsigned(emu::
 inline unsigned __match_any_sync(unsigned m, unsigned long long v) { return unsigned(emu::collective(emu::OP_MATCH64, m, v, 0)); }
 inline unsigned __reduce_max_sync(unsigned m, unsigned v) { return unsigned(emu::collective(emu::OP_RMAX, m, v, 0)); }
 inline unsigned __reduce_min_sync(unsigned m, unsigned v) { return unsigned(emu::collective(emu::OP_RMIN, m, v, 0)); }
+// the int overloads compare signed (k_cell_extent reduces cell coordinates): flipping the sign bit maps int order onto unsigned order
+inline int __reduce_max_sync(unsigned m, int v) { return int(__reduce_max_sync(m, unsigned(v) ^ 0x80000000u) ^ 0x80000000u); }
+inline int __reduce_min_sync(unsigned m, int v) { return int(__reduce_min_sync(m, unsigned(v) ^ 0x80000000u) ^ 0x80000000u); }
 
 // ---- scalar intrinsics
 inline unsigned __float_as_uint(float f) { unsigned u; std::memcpy(&u, &f, 4); return u; }

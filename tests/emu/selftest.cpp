@@ -25,7 +25,8 @@ __global__ void k_warp(unsigned *out) {                              // collecti
     const unsigned grp = __match_any_sync(0xffffffffu, lane / 8);
     const unsigned mx = __reduce_max_sync(0xffffffffu, lane * 7u % 32u), mn = __reduce_min_sync(0xffffffffu, lane + 5u);
     const unsigned up = __shfl_up_sync(0xffffffffu, lane, 1), dn = __shfl_down_sync(0xffffffffu, lane, 2), bc = __shfl_sync(0xffffffffu, lane * 10u, 3);
-    if (lane == 0) { unsigned *o = out + 8 * warp; o[0] = v; o[1] = ball; o[2] = grp; o[3] = mx; o[4] = mn; }
+    const int smx = __reduce_max_sync(0xffffffffu, lane < 4u ? -7 : (int)lane - 40), smn = __reduce_min_sync(0xffffffffu, (int)lane - 3);
+    if (lane == 0) { unsigned *o = out + 8 * warp; o[0] = v; o[1] = ball; o[2] = grp; o[3] = mx; o[4] = mn; out[16 + 2 * warp] = unsigned(smx); out[17 + 2 * warp] = unsigned(smn); }
     if (lane == 5) { unsigned *o = out + 8 * warp; o[5] = up; o[6] = dn; o[7] = bc; }
 }
 __global__ void k_partial(unsigned *out) {                           // partial masks, lanes that have exited
@@ -66,6 +67,7 @@ int main() {
             const unsigned *o = d + 8 * w;
             CHECK(o[0] == 32u * 33u / 2u); CHECK(o[1] == 0x49249249u); CHECK(o[2] == 0x000000ffu); CHECK(o[3] == 31u); CHECK(o[4] == 5u);
             CHECK(o[5] == 4u && o[6] == 7u && o[7] == 30u);
+            CHECK(int(d[16 + 2 * w]) == -7 && int(d[17 + 2 * w]) == -3);       // int overloads: signed order
         }
         cudaFree(d); }
     {   unsigned *d; cudaMalloc(&d, 8 * sizeof(unsigned)); cudaMemset(d, 0, 8 * sizeof(unsigned));

@@ -22,7 +22,10 @@ def _make_oracle(O, scene):
 
 
 def _pairset(p):
-    return {tuple(x) for x in p.tolist()}
+    """The ordered pairs as a set, once no pair has shown up in more than one manifold."""
+    pairs = [tuple(x) for x in p.tolist()]
+    assert len({tuple(sorted(x)) for x in pairs}) == len(pairs), "a pair has more than one manifold"
+    return set(pairs)
 
 
 @pytest.mark.parametrize("name", ["boxes", "chains"])

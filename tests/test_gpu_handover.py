@@ -88,7 +88,10 @@ def test_material_and_mass_patch(gpu, E, O):
 
 
 def _pairset(p):
-    return {tuple(x) for x in p.tolist()}
+    """The ordered pairs as a set, once no pair has shown up in more than one manifold."""
+    pairs = [tuple(x) for x in p.tolist()]
+    assert len({tuple(sorted(x)) for x in pairs}) == len(pairs), "a pair has more than one manifold"
+    return set(pairs)
 
 
 def _by_pair(c):

@@ -15,7 +15,10 @@ STEP_TOL = 1e-5
 
 
 def _pairset(p, ordered=True):
-    return {tuple(x) if ordered else tuple(sorted(x)) for x in p.tolist()}
+    """The pairs as a set, once no pair has shown up in more than one manifold."""
+    pairs = [tuple(x) for x in p.tolist()]
+    assert len({tuple(sorted(x)) for x in pairs}) == len(pairs), "a pair has more than one manifold"
+    return {x if ordered else tuple(sorted(x)) for x in pairs}
 
 
 def _by_pair(c):
