@@ -1194,33 +1194,52 @@ B2D_D float rel_speed(v3 J0, v3 J1, v3 J2, v3 J3, v3 vA, v3 wA, v3 vB, v3 wB) {
     return dot(J0, vA) + dot(J1, wA) + dot(J2, vB) + dot(J3, wB);
 }
 
+// Jacobian pieces of a contact point's rows, from (n, rA, rB): the normal row (n, J1, -n, J3) and the friction pair (t, T1,
+// -t, T3), (u, U1, -u, U3).  Every solver builds them with these two functions, so a piece computed once during the row
+// preparation and one rebuilt in a velocity pass are the same bits.
+struct FJac { v3 t, u, T1, T3, U1, U3; };
+B2D_D void normal_jac(v3 n, v3 rA, v3 rB, v3 &J1, v3 &J3) { J1 = cross(rA, n); J3 = -cross(rB, n); }
+B2D_D FJac friction_jac(v3 n, v3 rA, v3 rB) {
+    FJac f;
+    plane_space(n, f.t, f.u);
+    f.T1 = cross(rA, f.t); f.T3 = -cross(rB, f.t);
+    f.U1 = cross(rA, f.u); f.U3 = -cross(rB, f.u);
+    return f;
+}
+
 // contact_constraint::prepare (contact_constraint.cpp:15-56) + prepare_row of contact point slot mi: r0 = normal | rhs,
 // r1 = rA | eff_mass, r2 = rB | friction, r3 = eff_mass t0, t1, rhs t0, t1, im = warm-start impulses (n, t0, t1).
 // Row storage keeps (n, rA, rB) and rebuilds the Jacobian in registers: 84 B/point instead of the reference's 312 B
 // (constraint_row + _friction).  Shared by k_prepare_contacts, k_island_tiles and the restitution solver, so all produce
 // the same bits.  `restitution`: the rows of the restitution solver's groups (constraint_row_options{}, restitution_solver.cpp:
-// 146-310): no penetration error, the point's restitution always applied, no warm start.
+// 146-310): no penetration error, the point's restitution always applied, no warm start.  J1, J3 and fj receive the
+// Jacobian pieces the rows were prepared with.
 B2D_D void contact_point_rows(const Dev &d, size_t mi, const SBody &A, const SBody &B, v3 posA, q4 ornA, v3 posB, q4 ornB,
-                              float4 &r0, float4 &r1, float4 &r2, float4 &r3, float4 &imp, bool restitution = false) {
+                              float4 &r0, float4 &r1, float4 &r2, float4 &r3, float4 &imp, v3 &J1, v3 &J3, FJac &fj,
+                              bool restitution = false) {
     float4 a4 = d.pA[mi], b4 = d.pB[mi], n4 = d.pN[mi], im = restitution ? make_float4(0, 0, 0, 0) : d.pI[mi];
     v3 normal = mk3(n4);
     v3 pAw = to_world(mk3(a4), posA, ornA), pBw = to_world(mk3(b4), posB, ornB);
     v3 rA = pAw - posA, rB = pBw - posB;
-    v3 J1 = cross(rA, normal), J2 = -normal, J3 = -cross(rB, normal);
+    normal_jac(normal, rA, rB, J1, J3);
+    const v3 J2 = -normal;
     float em = eff_mass(normal, J1, J2, J3, A, B);
     float error = 0.0f;
     if (!restitution && a4.w > 0) error = a4.w / d.dt;
     float relvel = rel_speed(normal, J1, J2, J3, A.v, A.w, B.v, B.w);
     // solver.cpp:217-236: with the restitution solver on, the ordinary rows carry no restitution
     float rhs = -(error * 0.2f + relvel * (1.0f + (restitution ? n4.w : (d.rest_iters ? 0.0f : n4.w))));
-    v3 t, u; plane_space(normal, t, u);
-    v3 T1 = cross(rA, t), T2 = -t, T3 = -cross(rB, t);
-    v3 U1 = cross(rA, u), U2 = -u, U3 = -cross(rB, u);
-    float em_t = eff_mass(t, T1, T2, T3, A, B), em_u = eff_mass(u, U1, U2, U3, A, B);
-    float rhs_t = -rel_speed(t, T1, T2, T3, A.v, A.w, B.v, B.w), rhs_u = -rel_speed(u, U1, U2, U3, A.v, A.w, B.v, B.w);
+    fj = friction_jac(normal, rA, rB);
+    float em_t = eff_mass(fj.t, fj.T1, -fj.t, fj.T3, A, B), em_u = eff_mass(fj.u, fj.U1, -fj.u, fj.U3, A, B);
+    float rhs_t = -rel_speed(fj.t, fj.T1, -fj.t, fj.T3, A.v, A.w, B.v, B.w), rhs_u = -rel_speed(fj.u, fj.U1, -fj.u, fj.U3, A.v, A.w, B.v, B.w);
     r0 = f4(normal, rhs); r1 = f4(rA, em); r2 = f4(rB, b4.w);
     r3 = make_float4(em_t, em_u, rhs_t, rhs_u);
     imp = make_float4(im.x, im.y, im.z, 0);
+}
+B2D_D void contact_point_rows(const Dev &d, size_t mi, const SBody &A, const SBody &B, v3 posA, q4 ornA, v3 posB, q4 ornB,
+                              float4 &r0, float4 &r1, float4 &r2, float4 &r3, float4 &imp, bool restitution = false) {
+    v3 J1, J3; FJac fj;
+    contact_point_rows(d, mi, A, B, posA, ornA, posB, ornB, r0, r1, r2, r3, imp, J1, J3, fj, restitution);
 }
 
 // hinge_constraint::prepare, hinge_constraint.cpp:26-69 (no limits / springs / torque rows): the 7 row vectors of hinge h
@@ -1348,19 +1367,15 @@ __global__ void k_prepare_hinges(Dev d) {
 // __syncthreads between colours) and k_solve_df for the rest (per-body tickets in global memory).
 
 struct VBody { v3 dv, dw; float inv_m; m3 inv_I; uint32_t id; bool proc; float pad1, pad2; };
-// apply_row_impulse, constraint_row.cpp:24-32
+// apply_row_impulse, constraint_row.cpp:24-32, and the friction rows' (constraint_row_friction.cpp:47-53): the four
+// sums are independent, so their order does not matter.  SKIP_STATIC skips a static or kinematic side: its dv, dw start
+// at +0 with inv_m = 0, inv_I = 0, so for a finite impulse it could only receive (0 * J) * imp = +-0, and +0 + +-0 = +0;
+// nothing stores it either.  (rel_speed still reads it: dropping its terms could turn a -0 sum into +0.)  Only the
+// two-point tile skips: in the generic tile and the dataflow solve the branch costs more than it saves (more spills).
+template <bool SKIP_STATIC = false>
 B2D_D void apply_imp(VBody &A, VBody &B, v3 J0, v3 J1, v3 J2, v3 J3, float imp) {
-    A.dv += A.inv_m * J0 * imp;
-    B.dv += B.inv_m * J2 * imp;
-    A.dw += A.inv_I * J1 * imp;
-    B.dw += B.inv_I * J3 * imp;
-}
-// friction flavour keeps the reference's A-lin, A-ang, B-lin, B-ang order (constraint_row_friction.cpp:47-53)
-B2D_D void apply_imp_f(VBody &A, VBody &B, v3 J0, v3 J1, v3 J2, v3 J3, float imp) {
-    A.dv += A.inv_m * J0 * imp;
-    A.dw += A.inv_I * J1 * imp;
-    B.dv += B.inv_m * J2 * imp;
-    B.dw += B.inv_I * J3 * imp;
+    if (!SKIP_STATIC || A.proc) { A.dv += A.inv_m * J0 * imp; A.dw += A.inv_I * J1 * imp; }
+    if (!SKIP_STATIC || B.proc) { B.dv += B.inv_m * J2 * imp; B.dw += B.inv_I * J3 * imp; }
 }
 // solve(constraint_row&), constraint_row.cpp:38-57
 B2D_D float solve_row(float rhs, float em, float lo, float hi, float &impulse, float delta_relvel) {
@@ -1371,22 +1386,25 @@ B2D_D float solve_row(float rhs, float em, float lo, float hi, float &impulse, f
     else impulse = imp;
     return delta;
 }
-// one contact normal row; rows: r0 = normal | rhs, r1 = rA | eff_mass, r2 = rB | friction, im = impulses (n, t0, t1)
-B2D_D void nrow_solve(const float4 &r0, const float4 &r1, const float4 &r2, float4 &im, VBody &A, VBody &B, bool warm) {
-    v3 nrm = mk3(r0), rA = mk3(r1), rB = mk3(r2);
-    v3 J1 = cross(rA, nrm), J2 = -nrm, J3 = -cross(rB, nrm);
+// one contact normal row, Jacobian (n, J1, -n, J3); rhs and eff_mass from the rows, im = impulses (n, t0, t1)
+template <bool SKIP_STATIC = false>
+B2D_D void nrow_solve_j(v3 nrm, v3 J1, v3 J3, float rhs, float em, float4 &im, VBody &A, VBody &B, bool warm) {
+    const v3 J2 = -nrm;
     float delta;
     if (warm) delta = im.x;
-    else delta = solve_row(r0.w, r1.w, 0.0f, LARGE, im.x, rel_speed(nrm, J1, J2, J3, A.dv, A.dw, B.dv, B.dw));
-    apply_imp(A, B, nrm, J1, J2, J3, delta);
+    else delta = solve_row(rhs, em, 0.0f, LARGE, im.x, rel_speed(nrm, J1, J2, J3, A.dv, A.dw, B.dv, B.dw));
+    apply_imp<SKIP_STATIC>(A, B, nrm, J1, J2, J3, delta);
+}
+// the same from the rows r0 = normal | rhs, r1 = rA | eff_mass, r2 = rB | friction
+B2D_D void nrow_solve(const float4 &r0, const float4 &r1, const float4 &r2, float4 &im, VBody &A, VBody &B, bool warm) {
+    v3 J1, J3; normal_jac(mk3(r0), mk3(r1), mk3(r2), J1, J3);
+    nrow_solve_j(mk3(r0), J1, J3, r0.w, r1.w, im, A, B, warm);
 }
 // solve_friction, constraint_row_friction.cpp:11-54: both tangent candidates from one delta-velocity snapshot,
 // clamped to the circle of radius mu * lambda_n (lambda_n of THIS iteration); r3 = eff_mass t0, t1, rhs t0, t1
-B2D_D void frow_solve(const float4 &r0, const float4 &r1, const float4 &r2, const float4 &r3, float4 &im, VBody &A, VBody &B, bool warm) {
-    v3 nrm = mk3(r0), rA = mk3(r1), rB = mk3(r2);
-    v3 t, u; plane_space(nrm, t, u);
-    v3 T1 = cross(rA, t), T2 = -t, T3 = -cross(rB, t);
-    v3 U1 = cross(rA, u), U2 = -u, U3 = -cross(rB, u);
+template <bool SKIP_STATIC = false>
+B2D_D void frow_solve_j(const FJac &f, float mu, const float4 &r3, float4 &im, VBody &A, VBody &B, bool warm) {
+    const v3 t = f.t, u = f.u, T1 = f.T1, T2 = -f.t, T3 = f.T3, U1 = f.U1, U2 = -f.u, U3 = f.U3;
     float d0, d1;
     if (warm) { d0 = im.y; d1 = im.z; }
     else {
@@ -1394,7 +1412,7 @@ B2D_D void frow_solve(const float4 &r0, const float4 &r1, const float4 &r2, cons
         d1 = (r3.w - rel_speed(u, U1, U2, U3, A.dv, A.dw, B.dv, B.dw)) * r3.y;
         float i0 = im.y + d0, i1 = im.z + d1;
         float len_sqr = i0 * i0 + i1 * i1;
-        float max_len = r2.w * im.x;
+        float max_len = mu * im.x;
         if (len_sqr > max_len * max_len) {
             float len = sqrtf(len_sqr);
             if (len > EPS) { i0 = i0 / len * max_len; i1 = i1 / len * max_len; } else { i0 = 0; i1 = 0; }
@@ -1402,11 +1420,28 @@ B2D_D void frow_solve(const float4 &r0, const float4 &r1, const float4 &r2, cons
         }
         im.y = i0; im.z = i1;
     }
-    apply_imp_f(A, B, t, T1, T2, T3, d0);
-    apply_imp_f(A, B, u, U1, U2, U3, d1);
+    apply_imp<SKIP_STATIC>(A, B, t, T1, T2, T3, d0);
+    apply_imp<SKIP_STATIC>(A, B, u, U1, U2, U3, d1);
+}
+// the same from the rows r0 = normal | rhs, r1 = rA | eff_mass, r2 = rB | friction
+B2D_D void frow_solve(const float4 &r0, const float4 &r1, const float4 &r2, const float4 &r3, float4 &im, VBody &A, VBody &B, bool warm) {
+    frow_solve_j(friction_jac(mk3(r0), mk3(r1), mk3(r2)), r2.w, r3, im, A, B, warm);
+}
+B2D_D float &comp(v3 &v, int k) { return k == 0 ? v.x : (k == 1 ? v.y : v.z); }
+// m * v for a v whose k-th component is a zero: each row's dot without that term, the other two in dot's order
+B2D_D v3 mul_but(const m3 &m, v3 v, int k) {
+    auto d = [&](v3 r) { return k == 0 ? r.y * v.y + r.z * v.z : (k == 1 ? r.x * v.x + r.z * v.z : r.x * v.x + r.y * v.y); };
+    return mk3(d(m.r0), d(m.r1), d(m.r2));
 }
 // the five rows of a plain hinge (hinge_constraint.cpp:26-69): three point rows, two angular rows; r0..r6 as hinge_rows
-// writes them, the impulses repacked into r5 / r6 (unchanged by the warm start)
+// writes them, the impulses repacked into r5 / r6 (unchanged by the warm start).
+// LEAN (two-point tile) skips a static side (apply_imp<true>) and the structural zeros of the Jacobian: J0 = e_k,
+// J2 = -e_k, J1 and J3 with a zero k-th component in the point rows, J0 = J2 = 0 in the angular rows.  A velocity delta
+// starts at +0 and only ever receives sums, so it is never -0, and adding a +-0 term (0 * x for finite x) leaves it as it
+// is: dot(e_k, A.dv) = A.dv.k, a zero Jacobian component changes no component of dv, and a dot that drops its zero
+// term differs at most in the sign of a zero result, which the delta it is added to absorbs.  The bits are the same.
+// (dot(-e_k, B.dv) can be -0 where -B.dv.k is not, so the relative speed keeps that term.)
+template <bool LEAN = false>
 B2D_D void hinge_solve(const float4 &r0, const float4 &r1, const float4 &r2, const float4 &r3, const float4 &r4, float4 &r5, float4 &r6,
                        VBody &A, VBody &B, bool warm) {
     const v3 rA = mk3(r0), rB = mk3(r1), p = mk3(r2), q = mk3(r3);
@@ -1423,8 +1458,19 @@ B2D_D void hinge_solve(const float4 &r0, const float4 &r1, const float4 &r2, con
         } else { v3 ax = k == 3 ? p : q; J0 = mk3(0, 0, 0); J1 = ax; J2 = mk3(0, 0, 0); J3 = -ax; }
         float delta;
         if (warm) delta = imp[k];
-        else delta = solve_row(rhs[k], em[k], -SCALAR_MAX, SCALAR_MAX, imp[k], rel_speed(J0, J1, J2, J3, A.dv, A.dw, B.dv, B.dw));
-        apply_imp(A, B, J0, J1, J2, J3, delta);
+        else {
+            const float rv = LEAN && k < 3 ? comp(A.dv, k) + dot(J1, A.dw) + dot(J2, B.dv) + dot(J3, B.dw)
+                                           : rel_speed(J0, J1, J2, J3, A.dv, A.dw, B.dv, B.dw);
+            delta = solve_row(rhs[k], em[k], -SCALAR_MAX, SCALAR_MAX, imp[k], rv);
+        }
+        if (!LEAN) apply_imp(A, B, J0, J1, J2, J3, delta);
+        else if (k < 3) {
+            if (A.proc) { comp(A.dv, k) += A.inv_m * delta; A.dw += mul_but(A.inv_I, J1, k) * delta; }
+            if (B.proc) { comp(B.dv, k) -= B.inv_m * delta; B.dw += mul_but(B.inv_I, J3, k) * delta; }
+        } else {
+            if (A.proc) A.dw += A.inv_I * J1 * delta;
+            if (B.proc) B.dw += B.inv_I * J3 * delta;
+        }
     }
     r5 = make_float4(r5.x, r5.y, imp[0], imp[1]); r6 = make_float4(imp[2], imp[3], imp[4], 0);
 }
@@ -1820,10 +1866,32 @@ B2D_D void tile_error_max(uint32_t *s_err, uint32_t islot, float err) { if (err 
 //   generic:   joint rows [8..14], contact points 3-4 [15..24] (solver rows, then pA pB pN pL); the solver rows of points
 //              1-2 and the position-phase data of points 1-2 in registers;
 //   two-point: joint rows [10..16], the solver rows of point 2 in [5..9] during the velocity iterations (body records
-//              5-7 are idle then), pA pB pN pL of points 1-2 in [8..15] during the position iterations (the joint rows
-//              are dead then); only the solver rows of point 1 in registers.
+//              5-7 are idle then), the friction Jacobians of points 1-2 in [17..25] (tile_fjac_*), pA pB pN pL of
+//              points 1-2 in [8..15] during the position iterations (the joint rows are dead then); only the solver
+//              rows of point 1 in registers.  The two-point tile keeps every Jacobian piece of its contact rows from
+//              the row preparation: its solver rows hold n | rhs, J1 | eff_mass, J3 | friction in place of rA and rB,
+//              and the velocity passes do not rebuild them (plane_space, six cross products per point).
 constexpr size_t TILE_FUSED_SMEM = (8 + 7 + 10) * TILE_CAP * sizeof(float4);
-constexpr size_t TILE_FUSED_SMEM_2P = (8 + 2 + 7) * TILE_CAP * sizeof(float4);
+constexpr size_t TILE_FUSED_SMEM_2P = (8 + 2 + 7 + 9) * TILE_CAP * sizeof(float4);
+// friction Jacobian of contact point p (0, 1) of thread t's manifold, 18 floats: lane t of the float4 records 4p .. 4p + 3
+// from fj, and float2 p * TILE_CAP + t of the ninth record viewed as 2 TILE_CAP float2
+B2D_D void tile_fjac_store(float4 *fj, uint32_t t, int p, const FJac &f) {
+    float4 *q = fj + t;
+    q[(4 * p) * TILE_CAP] = make_float4(f.t.x, f.t.y, f.t.z, f.u.x);
+    q[(4 * p + 1) * TILE_CAP] = make_float4(f.u.y, f.u.z, f.T1.x, f.T1.y);
+    q[(4 * p + 2) * TILE_CAP] = make_float4(f.T1.z, f.T3.x, f.T3.y, f.T3.z);
+    q[(4 * p + 3) * TILE_CAP] = make_float4(f.U1.x, f.U1.y, f.U1.z, f.U3.x);
+    reinterpret_cast<float2 *>(fj + 8 * TILE_CAP)[p * TILE_CAP + t] = make_float2(f.U3.y, f.U3.z);
+}
+B2D_D FJac tile_fjac_load(const float4 *fj, uint32_t t, int p) {
+    const float4 *q = fj + t;
+    const float4 a = q[(4 * p) * TILE_CAP], b = q[(4 * p + 1) * TILE_CAP], c = q[(4 * p + 2) * TILE_CAP], e = q[(4 * p + 3) * TILE_CAP];
+    const float2 g = reinterpret_cast<const float2 *>(fj + 8 * TILE_CAP)[p * TILE_CAP + t];
+    FJac f;
+    f.t = mk3(a.x, a.y, a.z); f.u = mk3(a.w, b.x, b.y); f.T1 = mk3(b.z, b.w, c.x); f.T3 = mk3(c.y, c.z, c.w);
+    f.U1 = mk3(e.x, e.y, e.z); f.U3 = mk3(e.w, g.x, g.y);
+    return f;
+}
 // solver_body (+ position, orientation, record slot) of body `id` of a tiled constraint during the row preparation: a
 // dynamic body from the records staged by slot, a static / kinematic one from global memory
 B2D_D void tile_solver_body(const Dev &d, const float4 *sb, uint32_t id, SBody &s, v3 &pos, q4 &orn, uint32_t &slot) {
@@ -1867,6 +1935,7 @@ B2D_D void island_tiles(const Dev &d, int vel_iters, int pos_iters) {
     extern __shared__ float4 s_tile[];
     float4 *s_body = s_tile, *s_hr = s_tile + (TWO ? 10 : 8) * TILE_CAP, *s_row = s_tile + 15 * TILE_CAP;
     float4 *s_p2 = s_tile + 5 * TILE_CAP + threadIdx.x, *s_pt = s_tile + 8 * TILE_CAP + threadIdx.x;       // two-point only
+    float4 *s_fj = s_tile + 17 * TILE_CAP;
     __shared__ uint32_t s_err[TILE_CAP], s_done[TILE_CAP], s_root[TILE_CAP];
     __shared__ uint32_t s_ncol[2];
     const uint32_t tile0 = TWO ? 0u : d.cnt->ntiles2, ntiles = TWO ? d.cnt->ntiles2 : d.cnt->ntiles, t = threadIdx.x;
@@ -1911,8 +1980,18 @@ B2D_D void island_tiles(const Dev &d, int vel_iters, int pos_iters) {
             // a two-point tile holds no manifold with more points: one that gains a third point sets graph_changed
             // (np_merge) and the rebuild moves its island to a generic tile before the next solve
             ch = make_uint4(body_tag(pr.x, A), body_tag(pr.y, B), TWO ? min(npts, 2u) : npts, slot_pair(sa, sb));
-            contact_point_rows(d, m, A, B, posA, ornA, posB, ornB, a0, a1, a2, a3, aim);
-            if (npts > 1) contact_point_rows(d, NM + m, A, B, posA, ornA, posB, ornB, b0, b1, b2, b3, bim);
+            if (TWO) {      // rA, rB give way to the normal row's J1, J3; the friction Jacobians go to s_fj
+                v3 J1, J3; FJac fj;
+                contact_point_rows(d, m, A, B, posA, ornA, posB, ornB, a0, a1, a2, a3, aim, J1, J3, fj);
+                a1 = f4(J1, a1.w); a2 = f4(J3, a2.w); tile_fjac_store(s_fj, t, 0, fj);
+                if (npts > 1) {
+                    contact_point_rows(d, NM + m, A, B, posA, ornA, posB, ornB, b0, b1, b2, b3, bim, J1, J3, fj);
+                    b1 = f4(J1, b1.w); b2 = f4(J3, b2.w); tile_fjac_store(s_fj, t, 1, fj);
+                }
+            } else {
+                contact_point_rows(d, m, A, B, posA, ornA, posB, ornB, a0, a1, a2, a3, aim);
+                if (npts > 1) contact_point_rows(d, NM + m, A, B, posA, ornA, posB, ornB, b0, b1, b2, b3, bim);
+            }
             if (!TWO) for (uint32_t s = 2; s < npts; ++s) {
                 float4 *r = s_row + (s - 2) * 5 * TILE_CAP + t;
                 contact_point_rows(d, s * NM + m, A, B, posA, ornA, posB, ornB, r[0], r[TILE_CAP], r[2 * TILE_CAP], r[3 * TILE_CAP], r[4 * TILE_CAP]);
@@ -1925,6 +2004,50 @@ B2D_D void island_tiles(const Dev &d, int vel_iters, int pos_iters) {
         if (TWO && ch.z > 1) { s_p2[0] = b0; s_p2[TILE_CAP] = b1; s_p2[2 * TILE_CAP] = b2; s_p2[3 * TILE_CAP] = b3; s_p2[4 * TILE_CAP] = bim; }
         __syncthreads();
         const uint32_t nhc = s_ncol[0], ncc = s_ncol[1];
+        // the normal rows and the friction rows of this thread's manifold
+        auto normals = [&](VBody &A, VBody &B, bool warm) {
+            if (TWO) {
+                nrow_solve_j<true>(mk3(a0), mk3(a1), mk3(a2), a0.w, a1.w, aim, A, B, warm);
+                if (ch.z > 1) {
+                    const float4 r0 = s_p2[0], r1 = s_p2[TILE_CAP], r2 = s_p2[2 * TILE_CAP];
+                    float4 im = s_p2[4 * TILE_CAP];
+                    nrow_solve_j<true>(mk3(r0), mk3(r1), mk3(r2), r0.w, r1.w, im, A, B, warm);
+                    s_p2[4 * TILE_CAP] = im;
+                }
+            } else {
+                nrow_solve(a0, a1, a2, aim, A, B, warm);
+                if (ch.z > 1) nrow_solve(b0, b1, b2, bim, A, B, warm);
+                for (uint32_t s = 2; s < ch.z; ++s) {
+                    float4 *r = s_row + (s - 2) * 5 * TILE_CAP + t;
+                    float4 im = r[4 * TILE_CAP];
+                    nrow_solve(r[0], r[TILE_CAP], r[2 * TILE_CAP], im, A, B, warm);
+                    r[4 * TILE_CAP] = im;
+                }
+            }
+        };
+        auto frictions = [&](VBody &A, VBody &B, bool warm) {
+            if (TWO) {
+                frow_solve_j<true>(tile_fjac_load(s_fj, t, 0), a2.w, a3, aim, A, B, warm);
+                if (ch.z > 1) {
+                    float4 im = s_p2[4 * TILE_CAP];
+                    frow_solve_j<true>(tile_fjac_load(s_fj, t, 1), s_p2[2 * TILE_CAP].w, s_p2[3 * TILE_CAP], im, A, B, warm);
+                    s_p2[4 * TILE_CAP] = im;
+                }
+            } else {
+                frow_solve(a0, a1, a2, a3, aim, A, B, warm);
+                if (ch.z > 1) frow_solve(b0, b1, b2, b3, bim, A, B, warm);
+                for (uint32_t s = 2; s < ch.z; ++s) {
+                    float4 *r = s_row + (s - 2) * 5 * TILE_CAP + t;
+                    float4 im = r[4 * TILE_CAP];
+                    frow_solve(r[0], r[TILE_CAP], r[2 * TILE_CAP], r[3 * TILE_CAP], im, A, B, warm);
+                    r[4 * TILE_CAP] = im;
+                }
+            }
+        };
+        // With one contact colour a dynamic body has at most one tiled manifold, so its friction pass follows its normal
+        // pass on the same thread: both run in one phase, the bodies staying in registers in between.  Two-point tiles
+        // only: in the generic kernel the fused phase adds spills.
+        const bool fuse = TWO && ncc == 1;
         // ---- velocity iterations
         for (int it = -1; it < vel_iters; ++it) {
             const bool warm = it < 0;
@@ -1934,7 +2057,7 @@ B2D_D void island_tiles(const Dev &d, int vel_iters, int pos_iters) {
                                  r4 = s_hr[4 * TILE_CAP + t];
                     float4 r5 = s_hr[5 * TILE_CAP + t], r6 = s_hr[6 * TILE_CAP + t];
                     VBody A, B; tf_load(s_body, hh.x, slot_a(hh.w), A); tf_load(s_body, hh.y, slot_b(hh.w), B);
-                    hinge_solve(r0, r1, r2, r3, r4, r5, r6, A, B, warm);
+                    hinge_solve<TWO>(r0, r1, r2, r3, r4, r5, r6, A, B, warm);
                     tf_store(s_body, slot_a(hh.w), A); tf_store(s_body, slot_b(hh.w), B);
                     if (!warm) { s_hr[5 * TILE_CAP + t] = r5; s_hr[6 * TILE_CAP + t] = r6; }
                 }
@@ -1943,39 +2066,16 @@ B2D_D void island_tiles(const Dev &d, int vel_iters, int pos_iters) {
             for (uint32_t c = 0; c < ncc; ++c) {
                 if (ccol == c) {
                     VBody A, B; tf_load(s_body, ch.x, slot_a(ch.w), A); tf_load(s_body, ch.y, slot_b(ch.w), B);
-                    nrow_solve(a0, a1, a2, aim, A, B, warm);
-                    if (TWO && ch.z > 1) {
-                        float4 im = s_p2[4 * TILE_CAP];
-                        nrow_solve(s_p2[0], s_p2[TILE_CAP], s_p2[2 * TILE_CAP], im, A, B, warm);
-                        s_p2[4 * TILE_CAP] = im;
-                    }
-                    if (!TWO && ch.z > 1) nrow_solve(b0, b1, b2, bim, A, B, warm);
-                    if (!TWO) for (uint32_t s = 2; s < ch.z; ++s) {
-                        float4 *r = s_row + (s - 2) * 5 * TILE_CAP + t;
-                        float4 im = r[4 * TILE_CAP];
-                        nrow_solve(r[0], r[TILE_CAP], r[2 * TILE_CAP], im, A, B, warm);
-                        r[4 * TILE_CAP] = im;
-                    }
+                    normals(A, B, warm);
+                    if (fuse) frictions(A, B, warm);
                     tf_store(s_body, slot_a(ch.w), A); tf_store(s_body, slot_b(ch.w), B);
                 }
                 __syncthreads();
             }
-            for (uint32_t c = 0; c < ncc; ++c) {
+            if (!fuse) for (uint32_t c = 0; c < ncc; ++c) {
                 if (ccol == c) {
                     VBody A, B; tf_load(s_body, ch.x, slot_a(ch.w), A); tf_load(s_body, ch.y, slot_b(ch.w), B);
-                    frow_solve(a0, a1, a2, a3, aim, A, B, warm);
-                    if (TWO && ch.z > 1) {
-                        float4 im = s_p2[4 * TILE_CAP];
-                        frow_solve(s_p2[0], s_p2[TILE_CAP], s_p2[2 * TILE_CAP], s_p2[3 * TILE_CAP], im, A, B, warm);
-                        s_p2[4 * TILE_CAP] = im;
-                    }
-                    if (!TWO && ch.z > 1) frow_solve(b0, b1, b2, b3, bim, A, B, warm);
-                    if (!TWO) for (uint32_t s = 2; s < ch.z; ++s) {
-                        float4 *r = s_row + (s - 2) * 5 * TILE_CAP + t;
-                        float4 im = r[4 * TILE_CAP];
-                        frow_solve(r[0], r[TILE_CAP], r[2 * TILE_CAP], r[3 * TILE_CAP], im, A, B, warm);
-                        r[4 * TILE_CAP] = im;
-                    }
+                    frictions(A, B, warm);
                     tf_store(s_body, slot_a(ch.w), A); tf_store(s_body, slot_b(ch.w), B);
                 }
                 __syncthreads();
