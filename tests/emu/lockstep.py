@@ -1,8 +1,6 @@
-"""TEST INFRASTRUCTURE.  The library's CUDA kernels, executed by the CPU emulation (tests/emu), in lock step with the
-oracle through the normal Python adapter and C ABI -- the same comparison tests/test_gpu_parity.py makes on the GPU: ordered
-pair lists identical as multisets (a pair with two manifolds is a difference), post-solve state within 1e-5 (here: identical, glibc's sinf / cosf on both sides) with the oracle
-replaying the device's Gauss-Seidel order, manifolds and joint impulses re-synchronised every step.  The -m gpu lock-step
-tests (test_gpu_tile_edges.py, test_gpu_random_lockstep.py) call `lockstep` in-process, on the GPU or the emulation.
+"""TEST INFRASTRUCTURE.  The command-line driver of the CPU emulation (tests/emu): the library's CUDA kernels, executed by
+the emulation, in lock step with the oracle through the normal Python adapter and C ABI -- the comparison of
+tests/parity.py, which the -m gpu tests make on the GPU (here the state is identical: glibc's sinf / cosf on both sides).
 
     python tests/emu/lockstep.py fixed|narrow|wide|large|beyond FIRST LAST [--tiles 0|1] [--steps N] [--restitution] [--mutate]
                                  [--bp-warp-max N]     -> one JSON line
@@ -14,99 +12,12 @@ import json
 import os
 import sys
 import time
-from collections import Counter
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
 
-
-# How the device runs the step: plain launches that rebuild the islands every step, CUDA graphs that skip the rebuild while
-# the constraint graph is unchanged, and everything on the dataflow path (no island tiles).  The emulation launches plainly.
-MODES = {"plain": dict(B2D_GRAPH="0", B2D_GRAPH_REUSE="1", B2D_TILES="1"),
-         "graph": dict(B2D_GRAPH="1", B2D_GRAPH_REUSE="1", B2D_TILES="1"),
-         "dataflow": dict(B2D_GRAPH="0", B2D_GRAPH_REUSE="1", B2D_TILES="0")}
-STATE_KEYS = ("pos", "orn", "linvel", "angvel", "aabb")
-
-
-def build_world(E, scene, mode=None, env=None, **kw):
-    """E.scenes.build_world with the environment of `mode` (read when the world is created) and the extra variables `env`;
-    None: as the environment is."""
-    env = {**(MODES[mode] if mode is not None else {}), **(env or {})}
-    if not env:
-        return E.scenes.build_world(scene, **kw)
-    saved = {k: os.environ.get(k) for k in env}
-    os.environ.update(env)
-    try:
-        return E.scenes.build_world(scene, **kw)
-    finally:
-        for k, v in saved.items():
-            if v is None:
-                os.environ.pop(k, None)
-            else:
-                os.environ[k] = v
-
-
-def lockstep(E, O, scene, steps, restitution_solver=False, mode=None, hook=None, vel_iters=None, pos_iters=None, env=None,
-             before=None, max_bodies=None):
-    """One device world in `mode` (a key of MODES; None: as the environment says) against the oracle, `steps` single
-    steps.  vel_iters / pos_iters override the scene's settings on both sides; env: more environment variables for the
-    world's creation; hook(step, world) runs after each step's comparison (and may assert); before(step, world, oracle)
-    runs before each step, may change both worlds and returns the oracle to continue with; max_bodies reserves room for
-    bodies added on the way.  Returns ok, worst (largest state difference), exact (bit-identical steps), points (contact
-    points at the end), max_points (most points in one manifold at any step), flags, and digests: one hash of the device
-    state and ordered pair set per step, for comparing modes."""
-    import hashlib
-    import numpy as np
-    st = dict(scene["settings"])
-    if vel_iters is not None:
-        st["velocity_iterations"] = vel_iters
-    if pos_iters is not None:
-        st["position_iterations"] = pos_iters
-    w = build_world(E, scene, mode, env, flags=E.world.FLAG_RESTITUTION_SOLVER if restitution_solver else 0, max_bodies=max_bodies, **st)
-    o = O.OracleWorld(vel_iters=st["velocity_iterations"], pos_iters=st["position_iterations"])
-    if restitution_solver:
-        o.set_restitution_iterations(8, 3)          # no graph order handed over: the oracle's defaults are the device's conventions
-    o.add_bodies(scene["bodies"])
-    if scene["hinges"]:
-        h = scene["hinges"]
-        o.add_hinges(h["a"], h["b"], h["pivot_a"], h["pivot_b"], h["axis_a"], h["axis_b"])
-    if scene["exclusions"] is not None:
-        o.add_exclusions(*scene["exclusions"])
-    worst, exact, max_points, digests = 0.0, 0, 0, []
-    for s in range(steps):
-        if before is not None:
-            o = before(s, w, o)
-        w.step(1)
-        hi, pr = w.solver_order()
-        o.run_phases(O.PH_BROAD | O.PH_NARROW | O.PH_ISLANDS)
-        o.set_order(hi, pr)
-        o.run_phases(O.PH_SOLVE)
-        g, c = w.download_state(), o.state()
-        wp = w.pairs()
-        if Counter(map(tuple, wp.tolist())) != Counter(map(tuple, o.pairs().tolist())):
-            return dict(ok=False, step=s, why="ordered broadphase pair lists differ")
-        if not np.array_equal(w.islands(), o.islands()):
-            return dict(ok=False, step=s, why="island labels differ")
-        err = max(float(np.abs(g[k] - c[k]).max()) for k in STATE_KEYS)
-        worst = max(worst, err)
-        exact += err == 0.0
-        if err > 1e-5:
-            return dict(ok=False, step=s, why=f"state differs by {err:.3e}")
-        wp = wp[np.lexsort((wp[:, 1], wp[:, 0]))] if len(wp) else wp
-        digests.append(hashlib.sha1(b"".join(np.ascontiguousarray(x).tobytes() for x in [g[k] for k in STATE_KEYS] + [wp])).hexdigest())
-        o.set_state(g["pos"], g["orn"], g["linvel"], g["angvel"])
-        gc = w.contacts()
-        max_points = max(max_points, int(gc["num"].max(initial=0)))
-        o.set_contacts(gc["pairs"], gc["num"], gc["pts"], gc["att"], gc["lifetime"])
-        if scene["hinges"]:
-            o.set_hinge_impulses(w.hinge_impulses())
-        if hook is not None:
-            hook(s, w)
-    stats = w.stats()
-    w.close()
-    return dict(ok=stats["error_flags"] == 0, worst=worst, exact=exact, points=int(stats["contact_points"]), max_points=max_points,
-                flags=int(stats["error_flags"]), reused=int(stats["steps_reused"]), colors=int(stats["contact_colors"]), digests=digests)
+from tests.parity import build_world, lockstep  # noqa: E402
 
 
 def over_the_limit(E, scene, steps, restitution_solver=False):
@@ -124,69 +35,46 @@ def over_the_limit(E, scene, steps, restitution_solver=False):
     return dict(ok=True, flags=flags, raised=raised)
 
 
-def lockstep_with_mutations(E, O, scene, steps, seed):
-    """Same comparison while user code interferes every 13th step: b2d_remove_bodies, b2d_remove_exclusions, b2d_add_bodies,
-    b2d_upload_bodies (a patched velocity)."""
+def mutations(E, scene, seed, events):
+    """before(step, world, oracle) for `lockstep`: user code interferes every 13th step with b2d_remove_bodies,
+    b2d_remove_exclusions, b2d_add_bodies or b2d_upload_bodies (a patched velocity), on both sides; each is appended to
+    `events`.  Needs room for 16 more bodies."""
     import numpy as np
     R = E.rigidbody
     rng = np.random.default_rng(seed)
-    st = scene["settings"]
     nb = len(scene["bodies"]["kind"])
-    w = E.scenes.build_world(scene, max_bodies=nb + 16)
-    o = O.OracleWorld(vel_iters=st["velocity_iterations"], pos_iters=st["position_iterations"])
-    o.add_bodies(scene["bodies"])
-    if scene["hinges"]:
-        h = scene["hinges"]
-        o.add_hinges(h["a"], h["b"], h["pivot_a"], h["pivot_b"], h["axis_a"], h["axis_b"])
-    if scene["exclusions"] is not None:
-        o.add_exclusions(*scene["exclusions"])
     kind = np.asarray(scene["bodies"]["kind"]).copy()
     alive = np.ones(len(kind), bool)
     excluded = list(zip(*[x.tolist() for x in scene["exclusions"]])) if scene["exclusions"] is not None else []
-    events = 0
-    for s in range(steps):
-        if s and s % 13 == 0:
-            what, movable = rng.integers(4), np.where(alive & (kind == 0))[0]
-            if what == 0 and len(movable) > 4:
-                b = int(rng.choice(movable))
-                w.remove_bodies([b]); o.remove_bodies([b]); alive[b] = False
-            elif what == 1 and excluded:
-                a, b = excluded.pop()
-                if alive[a] and alive[b]:
-                    w.remove_exclusions([a], [b]); o.remove_exclusions([a], [b])
-            elif what == 3 and len(kind) < nb + 16:
-                d = R.RigidBodyDef(position=tuple(rng.uniform([-1, 2, -1], [1, 4, 1])), mass=float(rng.choice([0.5, 1.0, 2.0])), linvel=tuple(rng.uniform(-2, 2, 3)),
-                                   shape=[R.sphere_shape(0.3), R.box_shape((0.3, 0.2, 0.25)), R.capsule_shape(0.15, 0.3, 1)][rng.integers(3)])
-                soa = R.bodies_soa([d])
-                w.add_bodies(soa); o.add_bodies(soa)
-                kind, alive = np.append(kind, 0), np.append(alive, True)
-            else:
-                b = int(rng.choice(movable))
-                lv, av = rng.uniform(-3, 3, (1, 3)).astype(np.float32), rng.uniform(-3, 3, (1, 3)).astype(np.float32)
-                w.upload_bodies([b], linvel=lv, angvel=av)
-                x = o.state()
-                x["linvel"][b], x["angvel"][b] = lv[0], av[0]
-                o.set_state(x["pos"], x["orn"], x["linvel"], x["angvel"])
-            events += 1
-        w.step(1)
-        hi, pr = w.solver_order()
-        o.run_phases(O.PH_BROAD | O.PH_NARROW | O.PH_ISLANDS)
-        o.set_order(hi, pr)
-        o.run_phases(O.PH_SOLVE)
-        g, c = w.download_state(), o.state()
-        if Counter(map(tuple, w.pairs().tolist())) != Counter(map(tuple, o.pairs().tolist())):
-            return dict(ok=False, step=s, why="ordered broadphase pair lists differ")
-        err = max(float(np.abs(g[k][alive] - c[k][alive]).max()) for k in ("pos", "orn", "linvel", "angvel"))
-        if err > 1e-5:
-            return dict(ok=False, step=s, why=f"state differs by {err:.3e}")
-        o.set_state(g["pos"], g["orn"], g["linvel"], g["angvel"])
-        gc = w.contacts()
-        o.set_contacts(gc["pairs"], gc["num"], gc["pts"], gc["att"], gc["lifetime"])
-        if scene["hinges"]:
-            o.set_hinge_impulses(w.hinge_impulses())
-    flags = int(w.stats()["error_flags"])
-    w.close()
-    return dict(ok=flags == 0, worst=0.0, points=events, flags=flags)
+
+    def before(s, w, o):
+        nonlocal kind, alive
+        if not s or s % 13:
+            return o
+        what, movable = rng.integers(4), np.where(alive & (kind == 0))[0]
+        if what == 0 and len(movable) > 4:
+            b = int(rng.choice(movable))
+            w.remove_bodies([b]); o.remove_bodies([b]); alive[b] = False
+        elif what == 1 and excluded:
+            a, b = excluded.pop()
+            if alive[a] and alive[b]:
+                w.remove_exclusions([a], [b]); o.remove_exclusions([a], [b])
+        elif what == 3 and len(kind) < nb + 16:
+            d = R.RigidBodyDef(position=tuple(rng.uniform([-1, 2, -1], [1, 4, 1])), mass=float(rng.choice([0.5, 1.0, 2.0])), linvel=tuple(rng.uniform(-2, 2, 3)),
+                               shape=[R.sphere_shape(0.3), R.box_shape((0.3, 0.2, 0.25)), R.capsule_shape(0.15, 0.3, 1)][rng.integers(3)])
+            soa = R.bodies_soa([d])
+            w.add_bodies(soa); o.add_bodies(soa)
+            kind, alive = np.append(kind, 0), np.append(alive, True)
+        else:
+            b = int(rng.choice(movable))
+            lv, av = rng.uniform(-3, 3, (1, 3)).astype(np.float32), rng.uniform(-3, 3, (1, 3)).astype(np.float32)
+            w.upload_bodies([b], linvel=lv, angvel=av)
+            x = o.state()
+            x["linvel"][b], x["angvel"][b] = lv[0], av[0]
+            o.set_state(x["pos"], x["orn"], x["linvel"], x["angvel"])
+        events.append((s, int(what)))
+        return o
+    return before
 
 
 def free_run_against_real_stepper(E, O):
@@ -240,7 +128,13 @@ def main():
             res["large"], res["want"] = L.large_dynamic(scene["bodies"]).tolist(), scene["large"]
         else:
             scene = fixed[i]() if kind == "fixed" else (random_scene_wide if kind == "wide" else random_scene)(E, O, i)
-            res = lockstep_with_mutations(E, O, scene, steps, i) if "--mutate" in sys.argv else lockstep(E, O, scene, steps, restitution, mode)
+            if "--mutate" in sys.argv:
+                events = []
+                res = lockstep(E, O, scene, steps, restitution, mode, before=mutations(E, scene, i, events),
+                               max_bodies=len(scene["bodies"]["kind"]) + 16)
+                res["events"] = len(events)
+            else:
+                res = lockstep(E, O, scene, steps, restitution, mode)
         res.pop("digests", None)
         res["scene"] = scene["name"]
         out.append(res)

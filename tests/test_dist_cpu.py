@@ -1,10 +1,11 @@
 """The N > 1 path on CPU: island-aware partitioning, sub-scene extraction and the per-step bounds exchange, with a real
 two-process torch.distributed group on the gloo backend (127.0.0.1)."""
 import os
-import socket
 
 import numpy as np
 import pytest
+
+from tests.parity import free_port
 
 f32 = np.float32
 
@@ -54,14 +55,6 @@ def test_overlapping_ranks():
     assert dist.overlapping_ranks(b, margin=0.001) == []
 
 
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
 def _worker(rank, world_size, port, q):
     import torch.distributed as dist_mod
     import edyn_b200 as E
@@ -94,7 +87,7 @@ def test_bounds_exchange_gloo_world_size_2():
     import torch.multiprocessing as mp
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    port = _free_port()
+    port = free_port()
     procs = [ctx.Process(target=_worker, args=(r, 2, port, q)) for r in range(2)]
     for p in procs:
         p.start()
@@ -141,7 +134,7 @@ def test_island_migration_gloo_world_size_2(E):
     from tests._oracle_world import OracleBackedWorld
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    port = _free_port()
+    port = free_port()
     procs = [ctx.Process(target=_migration_worker, args=(r, 2, port, q)) for r in range(2)]
     for p in procs:
         p.start()
@@ -208,7 +201,7 @@ def test_chain_islands_migrate_with_joints_and_exclusions(E):
     from tests._oracle_world import OracleBackedWorld
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    port = _free_port()
+    port = free_port()
     procs = [ctx.Process(target=_chain_migration_worker, args=(r, 2, port, q)) for r in range(2)]
     for p in procs:
         p.start()
@@ -261,7 +254,7 @@ def test_interleaved_ranks_do_not_migrate_without_island_contact():
     import torch.multiprocessing as mp
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    port = _free_port()
+    port = free_port()
     procs = [ctx.Process(target=_interleaved_worker, args=(r, 2, port, q)) for r in range(2)]
     for p in procs:
         p.start()
@@ -306,7 +299,7 @@ def test_three_ranks_lowest_destination_wins():
     import torch.multiprocessing as mp
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    port = _free_port()
+    port = free_port()
     procs = [ctx.Process(target=_three_rank_worker, args=(r, 3, port, q)) for r in range(3)]
     for p in procs:
         p.start()

@@ -68,7 +68,7 @@ def test_emulated_restitution_solver(O):
 def test_emulated_kernels_under_user_interference(O):
     """b2d_remove_bodies, b2d_add_bodies, b2d_remove_exclusions and b2d_upload_bodies every 13th step of random scenes."""
     for res in _run("narrow", 0, 2, steps=100, mutate=True):
-        assert res["ok"] and res["points"] >= 6, res
+        assert res["ok"] and res["events"] >= 6, res
 
 
 def test_emulated_kernels_against_the_real_stepper_directly(O):

@@ -20,7 +20,7 @@ from collections import Counter
 import numpy as np
 import pytest
 
-from tests.emu.lockstep import build_world
+from tests.parity import build_world
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 EMU = os.environ.get("B2D_EMU") == "1"

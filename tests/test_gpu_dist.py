@@ -1,31 +1,14 @@
 """GPU tests of the pieces the multi-GPU path adds: body removal (registry.destroy) against the oracle through the C
 ABI, and -- on a box with at least two GPUs -- island migration between two ranks over NCCL (SURVEY.md section 8e)."""
 import os
-import socket
 
 import numpy as np
 import pytest
 
+from tests import parity as P
+
 pytestmark = pytest.mark.gpu
 f32 = np.float32
-
-
-def _make_oracle(O, scene):
-    o = O.OracleWorld(vel_iters=scene["settings"]["velocity_iterations"], pos_iters=scene["settings"]["position_iterations"])
-    o.add_bodies(scene["bodies"])
-    if scene["hinges"]:
-        h = scene["hinges"]
-        o.add_hinges(h["a"], h["b"], h["pivot_a"], h["pivot_b"], h["axis_a"], h["axis_b"])
-    if scene["exclusions"] is not None:
-        o.add_exclusions(*scene["exclusions"])
-    return o
-
-
-def _pairset(p):
-    """The ordered pairs as a set, once no pair has shown up in more than one manifold."""
-    pairs = [tuple(x) for x in p.tolist()]
-    assert len({tuple(sorted(x)) for x in pairs}) == len(pairs), "a pair has more than one manifold"
-    return set(pairs)
 
 
 @pytest.mark.parametrize("name", ["boxes", "chains"])
@@ -34,44 +17,22 @@ def test_remove_bodies_matches_oracle(gpu, E, O, name):
     the device stays in lock step with the oracle (same check as test_lockstep_phase_parity) across the removal."""
     scene = E.scenes.boxes_on_plane(3, jitter=0.01) if name == "boxes" else E.scenes.hinge_chains(3, 4)
     w = E.scenes.build_world(scene)
-    o = _make_oracle(O, scene)
+    o = P.oracle_for(O, scene)
     n = scene["dynamic"]
     gone = np.array([1, 4, 5, n - 1], np.uint32)
     for s in range(60):
         if s == 25:
             w.remove_bodies(gone); o.remove_bodies(gone)
-        w.run_phases(E.world.PH_BROAD); o.run_phases(O.PH_BROAD)
-        gp = _pairset(w.pairs())
-        assert gp == _pairset(o.pairs()), f"step {s}: broadphase pair lists differ"
+        gp = P.broad(E, O, w, o, s)
         if s >= 25:
-            assert not any(a in gone or b in gone for a, b in gp), "a removed body still owns a manifold"
-        w.run_phases(E.world.PH_NARROW | E.world.PH_ISLANDS); o.run_phases(O.PH_NARROW | O.PH_ISLANDS)
-        gi, oi = w.islands(), o.islands()
-        assert np.array_equal(gi, oi), f"step {s}: island partition differs"
-        w.run_phases(E.world.PH_SOLVE)
-        hi, pr = w.solver_order()
-        o.set_order(hi, pr)
-        o.run_phases(O.PH_SOLVE)
-        g, c = w.download_state(), o.state()
-        live = np.ones(len(g["pos"]), bool)
-        if s >= 25:
-            live[gone] = False
-        for k in ("pos", "orn", "linvel", "angvel"):
-            assert np.abs(g[k][live] - c[k][live]).max() <= 1e-5, f"step {s}: {k}"
-        o.set_state(g["pos"], g["orn"], g["linvel"], g["angvel"])
-        gc = w.contacts()
-        o.set_contacts(gc["pairs"], gc["num"], gc["pts"], gc["att"], gc["lifetime"])
+            assert not np.isin(gp, gone).any(), "a removed body still owns a manifold"
+        P.narrow(E, O, w, o, s)
+        P.islands(E, O, w, o, s)
+        g, _ = P.solve(E, O, w, o, s)            # the removed bodies' slots are not compared
+        P.resync(o, w, s, g)
     assert w.stats()["error_flags"] == 0
     st = w.download_state()
     assert np.all(st["linvel"][gone] == 0), "a destroyed body no longer moves"
-
-
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
 
 
 def _migration_worker(rank, world_size, port, q):
@@ -113,7 +74,7 @@ def test_island_migration_two_gpus(gpu, E):
     import torch.multiprocessing as mp
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    port = _free_port()
+    port = P.free_port()
     procs = [ctx.Process(target=_migration_worker, args=(r, 2, port, q)) for r in range(2)]
     for p in procs:
         p.start()
@@ -158,29 +119,19 @@ def test_island_sleeping_matches_oracle(gpu, E, O, name):
     make, steps = SLEEP_SCENES[name]
     scene = make(E)
     w = E.scenes.build_world(scene, flags=E.world.FLAG_SLEEPING)
-    o = _make_oracle(O, scene)
-    o.set_sleeping(True)
+    o = P.oracle_for(O, scene, sleeping=True)
     n = scene["dynamic"]
     slept = woke = 0
     prev = np.zeros(n, bool)
     for s in range(steps):
-        w.run_phases(E.world.PH_BROAD); o.run_phases(O.PH_BROAD)
-        assert _pairset(w.pairs()) == _pairset(o.pairs()), f"step {s}: broadphase pair lists differ"
-        w.run_phases(E.world.PH_NARROW | E.world.PH_ISLANDS); o.run_phases(O.PH_NARROW | O.PH_ISLANDS)
-        assert np.array_equal(w.islands(), o.islands()), f"step {s}: island partition differs"
+        P.broad(E, O, w, o, s)
+        P.narrow(E, O, w, o, s)
+        P.islands(E, O, w, o, s)
         gs, os_ = w.sleeping(), o.sleeping()
         assert np.array_equal(gs, os_), f"step {s}: sleeping flags differ: {np.where(gs != os_)[0][:8]}"
         slept += int((gs[:n] & ~prev).sum()); woke += int((~gs[:n] & prev).sum()); prev = gs[:n].copy()
-        w.run_phases(E.world.PH_SOLVE)
-        hi, pr = w.solver_order()
-        o.set_order(hi, pr)
-        o.run_phases(O.PH_SOLVE)
-        g, c = w.download_state(), o.state()
-        for k in ("pos", "orn", "linvel", "angvel"):
-            assert np.abs(g[k] - c[k]).max() <= 1e-5, f"step {s}: {k}"
-        o.set_state(g["pos"], g["orn"], g["linvel"], g["angvel"])
-        gc = w.contacts()
-        o.set_contacts(gc["pairs"], gc["num"], gc["pts"], gc["att"], gc["lifetime"])
+        g, _ = P.solve(E, O, w, o, s)
+        P.resync(o, w, s, g)
     assert w.stats()["error_flags"] == 0
     assert slept >= (3 if name == "sleep_and_wake" else n), f"{name}: only {slept} fall-asleep events"
     if name == "sleep_and_wake":
@@ -210,10 +161,8 @@ def test_collision_exclusion_add_remove_clear_device(gpu, E, O):
                 E.clear_collision_exclusion(w, a)
                 for p in gone:
                     o.remove_exclusions([p[0]], [p[1]])
-        w.run_phases(E.world.PH_BROAD); o.run_phases(O.PH_BROAD)
-        got = _pairset(w.pairs())
-        assert got == _pairset(o.pairs())
-        return {tuple(sorted(p)) for p in got}
+        got = P.broad(E, O, w, o, ops)
+        return {tuple(sorted(p)) for p in got.tolist()}
     assert run([]) == {(0, 1), (0, 2), (1, 2)}
     assert run([("+", 0, 1), ("+", 0, 2)]) == {(1, 2)}
     assert run([("+", 0, 1), ("+", 0, 2), ("-", 1, 0)]) == {(0, 1), (1, 2)}
@@ -236,5 +185,5 @@ def test_issue_76_destroy_then_recreate_device(gpu, E):
     w.upload_state(pos, st["orn"], np.zeros_like(st["linvel"]), np.zeros_like(st["angvel"]))
     w.step(30)
     assert abs(w.download_state()["pos"][box, 1] - 0.5) < 1e-3
-    assert _pairset(w.pairs()) == {(box, f1)}
+    P.check_pairs("60", w.pairs(), [(box, f1)])
     assert w.stats()["error_flags"] == 0

@@ -1,13 +1,16 @@
 """Parity AT THE BENCHMARKED SIZES (BASELINE.json configs 2-5): the settled device state -- bodies, persistent contact
 manifolds with their warm-start impulses, joint impulses -- is loaded into the CPU oracle (exactly what bench.py's
-cpu_baseline leg does), then both sides step in lock step and every phase is compared: ordered broadphase pair list,
-contact sets (point counts, attachments, lifetimes bit-equal; pivots / normals / distances <= 1e-5), island partition,
-and the post-solve state <= 1e-5 with the oracle replaying the device's colour order (within a colour the constraints
-touch disjoint dynamic bodies, so the coloured parallel solve IS a serial sweep in that order)."""
+cpu_baseline leg does), then both sides step in lock step (tests/parity.py) and every phase is compared: ordered
+broadphase pair list, contact sets (point counts, attachments, lifetimes bit-equal; the point floats <= 1e-5), island
+partition, the post-solve state <= 1e-5 with the oracle replaying the device's colour order (within a colour the
+constraints touch disjoint dynamic bodies, so the coloured parallel solve IS a serial sweep in that order), and the
+post-solve contacts and joint impulses before they are copied into the oracle again."""
 import os
 
 import numpy as np
 import pytest
+
+from tests import parity as P
 
 pytestmark = pytest.mark.gpu
 STEP_TOL = 1e-5
@@ -22,34 +25,6 @@ FULL = {
 }
 
 
-def _keys(pairs):
-    p = np.asarray(pairs, np.uint64).reshape(-1, 2)
-    return (p[:, 0] << np.uint64(32)) | p[:, 1]
-
-
-def _oracle_from_device(O, scene, w):
-    o = O.OracleWorld(vel_iters=scene["settings"]["velocity_iterations"], pos_iters=scene["settings"]["position_iterations"],
-                      threads=os.cpu_count() or 1)
-    o.add_bodies(scene["bodies"])
-    if scene["hinges"]:
-        h = scene["hinges"]
-        o.add_hinges(h["a"], h["b"], h["pivot_a"], h["pivot_b"], h["axis_a"], h["axis_b"])
-        o.set_hinge_impulses(w.hinge_impulses())
-    if scene["exclusions"] is not None:
-        o.add_exclusions(*scene["exclusions"])
-    st = w.download_state(aabb=False)
-    o.set_state(st["pos"], st["orn"], st["linvel"], st["angvel"])
-    c = w.contacts()
-    o.set_contacts(c["pairs"], c["num"], c["pts"], c["att"], c["lifetime"])
-    return o
-
-
-def _same_partition(a, b):
-    """Island labels are names, not values: two labelings describe the same partition iff the label pairs are in bijection."""
-    pa = np.unique(np.stack([a.astype(np.int64), b.astype(np.int64)], 1), axis=0)
-    return len(np.unique(pa[:, 0])) == len(pa) and len(np.unique(pa[:, 1])) == len(pa)
-
-
 @pytest.mark.parametrize("name", list(FULL))
 def test_full_size_lockstep_parity(gpu, E, O, name):
     make, settle, mpb = FULL[name]
@@ -57,35 +32,10 @@ def test_full_size_lockstep_parity(gpu, E, O, name):
     n_all = len(scene["bodies"]["kind"])
     w = E.scenes.build_world(scene, max_manifolds=max(4096, int(mpb * n_all)))
     w.step(settle)
-    o = _oracle_from_device(O, scene, w)
-    exact = 0
+    o = P.oracle_for(O, scene, threads=os.cpu_count() or 1)
+    P.load(o, w)
     for s in range(LOCKSTEP):
-        w.run_phases(E.world.PH_BROAD); o.run_phases(O.PH_BROAD)
-        gk, ok = _keys(w.pairs()), _keys(o.pairs())
-        assert len(gk) == len(ok) and np.array_equal(np.sort(gk), np.sort(ok)), f"{name} step {s}: ordered broadphase pair lists differ"
-        w.run_phases(E.world.PH_NARROW); o.run_phases(O.PH_NARROW)
-        gc, oc = w.contacts(), o.contacts()
-        gi, oi = np.argsort(_keys(gc["pairs"])), np.argsort(_keys(oc["pairs"]))
-        assert np.array_equal(_keys(gc["pairs"])[gi], _keys(oc["pairs"])[oi])
-        assert np.array_equal(gc["num"][gi], oc["num"][oi]), f"{name} step {s}: contact point counts differ"
-        valid = np.arange(4)[None, :] < gc["num"][gi][:, None]
-        assert np.array_equal(gc["att"][gi][valid], oc["att"][oi][valid]) and np.array_equal(gc["lifetime"][gi][valid], oc["lifetime"][oi][valid])
-        assert np.abs(gc["pts"][gi][valid] - oc["pts"][oi][valid]).max(initial=0) <= STEP_TOL
-        w.run_phases(E.world.PH_ISLANDS); o.run_phases(O.PH_ISLANDS)
-        assert _same_partition(w.islands(), o.islands()), f"{name} step {s}: island partition differs"
-        w.run_phases(E.world.PH_SOLVE)
-        hi, pr = w.solver_order()
-        o.set_order(hi, pr)
-        o.run_phases(O.PH_SOLVE)
-        g, c = w.download_state(aabb=True), o.state()
-        errs = {k: float(np.abs(g[k] - c[k]).max()) for k in ("pos", "orn", "linvel", "angvel", "aabb")}
-        assert max(errs.values()) <= STEP_TOL, f"{name} step {s}: {errs}"
-        exact += all(v == 0.0 for v in errs.values())
-        o.set_state(g["pos"], g["orn"], g["linvel"], g["angvel"])
-        gc = w.contacts()
-        o.set_contacts(gc["pairs"], gc["num"], gc["pts"], gc["att"], gc["lifetime"])
-        if scene["hinges"]:
-            o.set_hinge_impulses(w.hinge_impulses())
+        P.phase_step(E, O, w, o, s, STEP_TOL, partition=True)
     st = w.stats()
     assert st["error_flags"] == 0, st
     assert st["contact_points"] > scene["dynamic"] // 4
@@ -96,15 +46,7 @@ def test_full_size_lockstep_parity(gpu, E, O, name):
 def _free_pair(E, O, scene, mpb):
     n_all = len(scene["bodies"]["kind"])
     w = E.scenes.build_world(scene, max_manifolds=max(4096, int(mpb * n_all)))
-    o = O.OracleWorld(vel_iters=scene["settings"]["velocity_iterations"], pos_iters=scene["settings"]["position_iterations"],
-                      threads=os.cpu_count() or 1)
-    o.add_bodies(scene["bodies"])
-    if scene["hinges"]:
-        h = scene["hinges"]
-        o.add_hinges(h["a"], h["b"], h["pivot_a"], h["pivot_b"], h["axis_a"], h["axis_b"])
-    if scene["exclusions"] is not None:
-        o.add_exclusions(*scene["exclusions"])
-    return w, o
+    return w, P.oracle_for(O, scene, threads=os.cpu_count() or 1)
 
 
 def _free_step(E, O, w, o):
@@ -112,10 +54,7 @@ def _free_step(E, O, w, o):
     in which rows are swept (any order is a valid Gauss-Seidel sweep; the reference's own order is EnTT's pool order,
     which SURVEY A.11 could not pin), so what accumulates is the floating-point difference of the whole pipeline."""
     w.run_phases(E.world.PH_ALL)
-    hi, pr = w.solver_order()
-    o.run_phases(O.PH_BROAD | O.PH_NARROW | O.PH_ISLANDS)
-    o.set_order(hi, pr)
-    o.run_phases(O.PH_SOLVE)
+    P.oracle_step(O, o, w)
 
 
 def _rel_err(w, o, n):
@@ -134,7 +73,7 @@ def test_chain_slice_1000_free_running_steps(gpu, E, O):
     rel, g, c = _rel_err(w, o, n)
     assert rel <= 1e-4, f"relative position error after 1000 steps {rel:.3e}"
     assert float(np.abs(g["linvel"][:n] - c["linvel"][:n]).max()) <= 1e-3
-    assert np.array_equal(np.sort(_keys(w.pairs())), np.sort(_keys(o.pairs())))
+    P.check_pairs(1000, w.pairs(), o.pairs())
     assert w.stats()["error_flags"] == 0
 
 

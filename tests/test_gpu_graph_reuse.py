@@ -3,37 +3,26 @@ while the constraint graph is unchanged.  The results must be the bits of plain 
 import numpy as np
 import pytest
 
+from tests.parity import build_world, same_state
+
 pytestmark = pytest.mark.gpu
 
 LINKS = 4
 
 
-def _world(E, scene, monkeypatch, graph, reuse=True):
-    with monkeypatch.context() as m:
-        m.setenv("B2D_GRAPH", "1" if graph else "0")
-        m.setenv("B2D_GRAPH_REUSE", "1" if reuse else "0")
-        return E.scenes.build_world(scene)
-
-
-def _same(a, b):
-    sa, sb = a.download_state(), b.download_state()
-    for k in ("pos", "orn", "linvel", "angvel", "aabb"):
-        assert np.array_equal(sa[k], sb[k]), k
-
-
 @pytest.mark.parametrize("timing", [True, False])
-def test_reused_rebuild_matches_plain_launches(gpu, E, monkeypatch, timing):
+def test_reused_rebuild_matches_plain_launches(gpu, E, timing):
     """A settled slice of the chains workload, 200 steps as graphs with reuse, as graphs without and as plain launches.
     Mid-run one chain is thrown upwards (its plane contacts break and re-form) and one body is removed."""
     scene = E.scenes.hinge_chains(16, 16, LINKS)
-    plain = _world(E, scene, monkeypatch, graph=False)
-    reuse = _world(E, scene, monkeypatch, graph=True)
-    full = _world(E, scene, monkeypatch, graph=True, reuse=False)
+    plain = build_world(E, scene, env=dict(B2D_GRAPH="0", B2D_GRAPH_REUSE="1"))
+    reuse = build_world(E, scene, env=dict(B2D_GRAPH="1", B2D_GRAPH_REUSE="1"))
+    full = build_world(E, scene, env=dict(B2D_GRAPH="1", B2D_GRAPH_REUSE="0"))
     worlds = (plain, reuse, full)
     for w in worlds:
         w.set_timing(timing)
         w.step(150)                                            # settle, as bench.py does
-    _same(plain, reuse); _same(plain, full)
+    same_state(plain, reuse, full)
 
     def counts():
         st = reuse.stats()
@@ -46,7 +35,7 @@ def test_reused_rebuild_matches_plain_launches(gpu, E, monkeypatch, timing):
     r1, u1 = counts()
     assert (r1 - r0) + (u1 - u0) == 60
     assert u1 - u0 >= 54, (r1 - r0, u1 - u0)
-    _same(plain, reuse); _same(plain, full)
+    same_state(plain, reuse, full)
 
     # throw chain 37 upwards: its manifolds with the plane are destroyed, then created again (with points, in the same
     # step) when it lands: at least two rebuilds, the other steps reuse
@@ -55,7 +44,7 @@ def test_reused_rebuild_matches_plain_launches(gpu, E, monkeypatch, timing):
     for w in worlds:
         w.upload_bodies(ids, linvel=up)
         w.step(70)
-    _same(plain, reuse); _same(plain, full)
+    same_state(plain, reuse, full)
     r2, u2 = counts()
     assert r2 - r1 >= 2 and u2 - u1 >= 50, (r2 - r1, u2 - u1)
 
@@ -68,7 +57,7 @@ def test_reused_rebuild_matches_plain_launches(gpu, E, monkeypatch, timing):
     assert r4 - r3 == 1
     for w in worlds:
         w.step(69)
-    _same(plain, reuse); _same(plain, full)
+    same_state(plain, reuse, full)
 
     st_r, st_f, st_p = reuse.stats(), full.stats(), plain.stats()
     assert st_f["steps_reused"] == 0 and st_f["steps_rebuilt"] == st_f["steps"]

@@ -5,25 +5,15 @@ island hand-over (b2d_island_halo / b2d_handover_plan / _pack / _unpack) driven 
 The hand-over is run twice: with ranks as THREADS sharing one device (always runs, so the driver's single-GPU box
 exercises the same library code) and with one process per GPU over NCCL (needs >= 2 GPUs)."""
 import os
-import socket
 import threading
 
 import numpy as np
 import pytest
 
+from tests import parity as P
+
 pytestmark = pytest.mark.gpu
 f32 = np.float32
-
-
-def _make_oracle(O, scene):
-    o = O.OracleWorld(vel_iters=scene["settings"]["velocity_iterations"], pos_iters=scene["settings"]["position_iterations"])
-    o.add_bodies(scene["bodies"])
-    if scene["hinges"]:
-        h = scene["hinges"]
-        o.add_hinges(h["a"], h["b"], h["pivot_a"], h["pivot_b"], h["axis_a"], h["axis_b"])
-    if scene["exclusions"] is not None:
-        o.add_exclusions(*scene["exclusions"])
-    return o
 
 
 # ----------------------------------------------------------------------------- CUDA graphs
@@ -83,46 +73,15 @@ def test_material_and_mass_patch(gpu, E, O):
     b = scene["bodies"]
     b["inv_mass"][ids] = f32(0.25); b["inv_inertia"][ids] *= f32(0.25); b["friction"][ids] = f32(0.1); b["restitution"][ids] = f32(0.3)
     w.upload_bodies(ids, inv_mass=b["inv_mass"][ids], inv_inertia=b["inv_inertia"][ids], friction=b["friction"][ids], restitution=b["restitution"][ids])
-    o = _make_oracle(O, scene)
+    o = P.oracle_for(O, scene)
     _lockstep(E, O, w, o, 40)
-
-
-def _pairset(p):
-    """The ordered pairs as a set, once no pair has shown up in more than one manifold."""
-    pairs = [tuple(x) for x in p.tolist()]
-    assert len({tuple(sorted(x)) for x in pairs}) == len(pairs), "a pair has more than one manifold"
-    return set(pairs)
-
-
-def _by_pair(c):
-    return {tuple(p): k for k, p in enumerate(c["pairs"].tolist())}
 
 
 def _lockstep(E, O, w, o, steps, before_step=None):
     for s in range(steps):
         if before_step:
             before_step(s)
-        w.run_phases(E.world.PH_BROAD); o.run_phases(O.PH_BROAD)
-        assert _pairset(w.pairs()) == _pairset(o.pairs()), f"step {s}: broadphase pair lists (body[0], body[1]) differ"
-        w.run_phases(E.world.PH_NARROW | E.world.PH_ISLANDS); o.run_phases(O.PH_NARROW | O.PH_ISLANDS)
-        assert np.array_equal(w.islands(), o.islands()), f"step {s}: island partition differs"
-        gc, oc = w.contacts(), o.contacts()
-        gi, oi = _by_pair(gc), _by_pair(oc)
-        assert gi.keys() == oi.keys()
-        for key, k in gi.items():
-            j = oi[key]
-            m = int(gc["num"][k])
-            assert m == oc["num"][j] and np.array_equal(gc["att"][k, :m], oc["att"][j, :m]), f"step {s}: contact set differs for {key}"
-        w.run_phases(E.world.PH_SOLVE)
-        hi, pr = w.solver_order()
-        o.set_order(hi, pr)
-        o.run_phases(O.PH_SOLVE)
-        g, c = w.download_state(), o.state()
-        for k in ("pos", "orn", "linvel", "angvel"):
-            assert np.abs(g[k] - c[k]).max() <= 1e-5, f"step {s}: {k} off by {np.abs(g[k] - c[k]).max()}"
-        o.set_state(g["pos"], g["orn"], g["linvel"], g["angvel"])
-        gc = w.contacts()
-        o.set_contacts(gc["pairs"], gc["num"], gc["pts"], gc["att"], gc["lifetime"])
+        P.phase_step(E, O, w, o, s)
     assert w.stats()["error_flags"] == 0
 
 
@@ -141,7 +100,7 @@ def test_kinematic_body_pushes_a_stack(gpu, E, O):
     b["inv_mass"][slab] = 0; b["inv_inertia"][slab] = 0; b["gravity"][slab] = 0
     b["linvel"][slab] = (0.6, 0, 0)
     w = E.scenes.build_world(scene)
-    o = _make_oracle(O, scene)
+    o = P.oracle_for(O, scene)
     dt = f32(1.0 / 60)
     pos = b["pos"][slab].copy()
 
@@ -168,7 +127,7 @@ def test_kind_patch_dynamic_to_kinematic(gpu, E, O):
     b = scene["bodies"]
     b["kind"][3] = KINEMATIC; b["inv_mass"][3] = 0; b["inv_inertia"][3] = 0
     w.upload_bodies([3], kind=[KINEMATIC])
-    o = _make_oracle(O, scene)
+    o = P.oracle_for(O, scene)
     _lockstep(E, O, w, o, 30)
 
 
@@ -191,9 +150,8 @@ def test_collision_filter_truth_table_device(gpu, E, O):
         soa["mask"] = np.array([full if ma is None else ma, full if mb is None else mb], np.uint64)
         w = E.World(2, max_manifolds=16); w.add_bodies(soa)
         o = O.OracleWorld(); o.add_bodies(soa)
-        w.run_phases(E.world.PH_BROAD); o.run_phases(O.PH_BROAD)
-        assert _pairset(w.pairs()) == _pairset(o.pairs()), (ga, ma, gb, mb)
-        assert (len(w.pairs()) == 1) == want, (ga, ma, gb, mb)
+        got = P.broad(E, O, w, o, (ga, ma, gb, mb))
+        assert (len(got) == 1) == want, (ga, ma, gb, mb)
 
 
 # ----------------------------------------------------------------------------- island hand-over
@@ -306,14 +264,6 @@ def test_chain_handover_carries_joints_and_exclusions(gpu, E):
     _check_chains(E, _run_threads("chains", 80))
 
 
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
 def _nccl_worker(rank, N, port, scene_name, steps, q):
     import traceback
     import torch
@@ -343,7 +293,7 @@ def test_handover_two_gpus_nccl(gpu, E, scene_name, steps):
     import torch.multiprocessing as mp
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    port = _free_port()
+    port = P.free_port()
     procs = [ctx.Process(target=_nccl_worker, args=(r, 2, port, scene_name, steps, q)) for r in range(2)]
     for p in procs:
         p.start()

@@ -9,7 +9,7 @@ class flips between steps (bodies added, a kind patch to static and back).
 
 Every step, in three modes (plain launches, CUDA graphs with rebuild reuse, dataflow only) and with both neighbourhood
 searches (warp per body, and thread per body: B2D_BP_WARP_MAX=0): the tile packing against its restatement
-(tests/tile_packing.py), the oracle lock step of tests/emu/lockstep.py, and all runs bit-identical to each other (state
+(tests/tile_packing.py), the oracle lock step of tests/parity.py, and all runs bit-identical to each other (state
 and ordered pair set).  Each test first asserts that its scene has the large dynamic bodies it was built for, by the
 host's rule restated in numpy.  Also runs against the CPU emulation (B2D_EMU=1: no graphs, fewer steps); the cases
 beyond the limits run there only (tests/test_emu_device.py)."""
@@ -20,7 +20,7 @@ import pytest
 
 from tests import large_scenes as L
 from tests import tile_packing as TP
-from tests.emu.lockstep import lockstep
+from tests.parity import lockstep, oracle_for, load, same_digests
 
 pytestmark = pytest.mark.gpu
 
@@ -72,10 +72,7 @@ def run_all(E, O, scene, steps=STEPS, modes=MODES, search=("warp", "thread"), **
             if mode == "dataflow":
                 assert rec.tiled_steps == 0
             out[(s, mode)] = (res, rec)
-    first = next(iter(out))
-    for k, (res, _) in out.items():
-        diff = [i for i, (a, b) in enumerate(zip(out[first][0]["digests"], res["digests"])) if a != b]
-        assert not diff, f"{scene['name']}: {k} differs from {first} from step {diff[0]} on"
+    same_digests({f"{scene['name']} {k}": res["digests"] for k, (res, _) in out.items()})
     return out
 
 
@@ -140,7 +137,6 @@ def drift_events(E, O, scene, arrivals, log):
     the crate is patched static, at step 40 dynamic again.  The oracle has no kind patch: it is rebuilt from the device's
     state with the new kinds and continues from the device's manifolds, as it does every step."""
     from edyn_b200.rigidbody import DYNAMIC, STATIC
-    st = scene["settings"]
     crate = scene["roots"]["crate"]
     bodies = {k: np.concatenate([np.asarray(scene["bodies"][k]), np.asarray(arrivals[k])]) for k in scene["bodies"]}
     n0 = len(scene["bodies"]["kind"])
@@ -151,10 +147,8 @@ def drift_events(E, O, scene, arrivals, log):
         b.update(pos=g["pos"], orn=g["orn"], linvel=g["linvel"], angvel=g["angvel"], kind=kind)
         if kind[crate] != DYNAMIC:
             b["inv_mass"][crate], b["inv_inertia"][crate] = 0, 0
-        o = O.OracleWorld(vel_iters=st["velocity_iterations"], pos_iters=st["position_iterations"])
-        o.add_bodies(b)
-        c = w.contacts()
-        o.set_contacts(c["pairs"], c["num"], c["pts"], c["att"], c["lifetime"])
+        o = oracle_for(O, dict(scene, bodies=b))
+        load(o, w, g)
         return o
 
     def before(s, w, o):
@@ -180,7 +174,7 @@ def test_large_class_flips_between_steps(gpu, E, O):
     follows a kind patch to static and back; the lock step holds through every change."""
     scene, arrivals = L.drift_scene(E), L.drift_arrivals(E)
     crate, steps = scene["roots"]["crate"], 60
-    digests = []
+    digests = {}
     for s in SEARCH:
         for mode in MODES:
             log = []
@@ -188,5 +182,5 @@ def test_large_class_flips_between_steps(gpu, E, O):
                            before=drift_events(E, O, scene, arrivals, log))
             assert res["ok"], (s, mode, res)
             assert [(k, crate in lg) for k, lg in log] == [(0, False), (5, True), (25, False), (40, True)], log
-            digests.append(res["digests"])
-    assert all(d == digests[0] for d in digests[1:])
+            digests[(s, mode)] = res["digests"]
+    same_digests(digests)

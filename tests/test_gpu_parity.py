@@ -8,32 +8,12 @@ import os
 import numpy as np
 import pytest
 
+from tests import parity as P
+
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 f32 = np.float32
 STEP_TOL = 1e-5
-
-
-def _pairset(p, ordered=True):
-    """The pairs as a set, once no pair has shown up in more than one manifold."""
-    pairs = [tuple(x) for x in p.tolist()]
-    assert len({tuple(sorted(x)) for x in pairs}) == len(pairs), "a pair has more than one manifold"
-    return {x if ordered else tuple(sorted(x)) for x in pairs}
-
-
-def _by_pair(c):
-    return {tuple(c["pairs"][k].tolist()): k for k in range(len(c["num"]))}
-
-
-def _make_oracle(O, scene, threads=1):
-    o = O.OracleWorld(vel_iters=scene["settings"]["velocity_iterations"], pos_iters=scene["settings"]["position_iterations"], threads=threads)
-    o.add_bodies(scene["bodies"])
-    if scene["hinges"]:
-        h = scene["hinges"]
-        o.add_hinges(h["a"], h["b"], h["pivot_a"], h["pivot_b"], h["axis_a"], h["axis_b"])
-    if scene["exclusions"] is not None:
-        o.add_exclusions(*scene["exclusions"])
-    return o
 
 
 # ----------------------------------------------------------------------------- golden vectors from the reference
@@ -53,7 +33,7 @@ def test_narrowphase_matches_reference_vectors(gpu, E):
     w.upload_contacts(pairs, np.zeros(n, np.uint32), np.zeros((n, 4, 18), f32), np.zeros((n, 4), np.uint32))
     w.run_phases(E.world.PH_NARROW)
     c = w.contacts()
-    idx = _by_pair(c)
+    idx = {tuple(p): k for k, p in enumerate(c["pairs"].tolist())}
     bad = 0
     for i in range(n):
         k = idx[(2 * i, 2 * i + 1)]
@@ -115,13 +95,13 @@ def test_broadphase_matches_reference_tree_vectors(gpu, E):
     g = np.load(os.path.join(GOLD, "broadphase.npz"))
     keys = [k[4:] for k in g.files if k.startswith("soa_")]
     off = po = 0
-    for n, c in zip(g["sizes"].tolist(), g["counts"].tolist()):
+    for i, (n, c) in enumerate(zip(g["sizes"].tolist(), g["counts"].tolist())):
         soa = {k: g["soa_" + k][off:off + n] for k in keys}
         w = E.World(n, max_manifolds=max(4096, 4 * c))
         w.add_bodies(soa)
         assert np.array_equal(w.download_state(aabb=True)["aabb"], g["aabb1"][off:off + n])
         w.run_phases(E.world.PH_BROAD)
-        assert _pairset(w.pairs()) == {tuple(p) for p in g["pairs"][po:po + c].tolist()}
+        P.check_pairs(f"0 of scene {i}", w.pairs(), g["pairs"][po:po + c])
         assert w.stats()["error_flags"] == 0
         off += n; po += c
 
@@ -145,35 +125,12 @@ def test_lockstep_phase_parity(gpu, E, O, name):
     make, steps = SCENES[name]
     scene = make(E)
     w = E.scenes.build_world(scene)
-    o = _make_oracle(O, scene)
+    o = P.oracle_for(O, scene)
     exact_steps = 0
     for s in range(steps):
-        w.run_phases(E.world.PH_BROAD); o.run_phases(O.PH_BROAD)
-        assert _pairset(w.pairs()) == _pairset(o.pairs()), f"step {s}: broadphase pair lists differ"
-        w.run_phases(E.world.PH_NARROW); o.run_phases(O.PH_NARROW)
-        gc, oc = w.contacts(), o.contacts()
-        gi, oi = _by_pair(gc), _by_pair(oc)
-        assert gi.keys() == oi.keys()
-        for key, k in gi.items():
-            j = oi[key]
-            assert gc["num"][k] == oc["num"][j], f"step {s}: point count differs for {key}"
-            m = int(gc["num"][k])
-            assert np.array_equal(gc["att"][k, :m], oc["att"][j, :m]) and np.array_equal(gc["lifetime"][k, :m], oc["lifetime"][j, :m])
-            assert np.abs(gc["pts"][k, :m] - oc["pts"][j, :m]).max(initial=0) <= STEP_TOL
-        w.run_phases(E.world.PH_ISLANDS); o.run_phases(O.PH_ISLANDS)
-        assert np.array_equal(w.islands(), o.islands()), f"step {s}: island partition differs"
-        w.run_phases(E.world.PH_SOLVE)
-        hi, pr = w.solver_order()
-        o.set_order(hi, pr)
-        o.run_phases(O.PH_SOLVE)
-        g, c = w.download_state(inv_IW=True), o.state()
-        errs = {k: float(np.abs(g[k] - c[k]).max()) for k in ("pos", "orn", "linvel", "angvel", "aabb")}
-        assert max(errs.values()) <= STEP_TOL, f"step {s}: {errs}"
+        # every step a fresh single-step comparison: the oracle continues from the device's bodies, contacts and joints
+        errs = P.phase_step(E, O, w, o, s, STEP_TOL)
         exact_steps += all(v == 0.0 for v in errs.values())
-        # continue from the device state (bodies and persistent contacts), so every step is a fresh single-step comparison
-        o.set_state(g["pos"], g["orn"], g["linvel"], g["angvel"])
-        gc = w.contacts()
-        o.set_contacts(gc["pairs"], gc["num"], gc["pts"], gc["att"], gc["lifetime"])
     assert w.stats()["error_flags"] == 0
     assert exact_steps >= steps // 2, f"only {exact_steps}/{steps} steps were bit-identical"
 
@@ -182,26 +139,16 @@ def test_solver_only_parity_from_injected_contacts(gpu, E, O):
     """Row preparation + warm start + velocity iterations + integration + position iterations in isolation: the same
     manifolds (with non-zero warm-start impulses) are injected on both sides."""
     scene = E.scenes.mixed_pile(5)
-    o = _make_oracle(O, scene)
+    o = P.oracle_for(O, scene)
     o.step(60)
     st, c = o.state(), o.contacts()
     assert c["num"].sum() > 100
     w = E.scenes.build_world(scene)
     w.upload_state(st["pos"], st["orn"], st["linvel"], st["angvel"])
     w.upload_contacts(c["pairs"], c["num"], c["pts"], c["att"], c["lifetime"])
-    w.run_phases(E.world.PH_ISLANDS | E.world.PH_SOLVE)
-    hi, pr = w.solver_order()
-    o.run_phases(O.PH_ISLANDS)
-    o.set_order(hi, pr)
-    o.run_phases(O.PH_SOLVE)
-    g, r = w.download_state(), o.state()
-    for k in ("pos", "orn", "linvel", "angvel"):
-        assert np.abs(g[k] - r[k]).max() <= STEP_TOL, k
-    gc, oc = w.contacts(), o.contacts()
-    gi, oi = _by_pair(gc), _by_pair(oc)
-    for key, k in gi.items():
-        m = int(gc["num"][k])
-        assert np.abs(gc["pts"][k, :m, 15:18] - oc["pts"][oi[key], :m, 15:18]).max(initial=0) <= 1e-5      # applied impulses
+    P.islands(E, O, w, o, 0)
+    P.solve(E, O, w, o, 0, STEP_TOL)
+    P.check_contacts(0, w.contacts(), o.contacts(), STEP_TOL)          # the applied impulses among them
 
 
 # ----------------------------------------------------------------------------- free-running trajectories
@@ -211,7 +158,7 @@ def test_hello_world_1000_steps(gpu, E, O):
     FREE here, in its own natural Gauss-Seidel order."""
     scene = E.scenes.hello_world()
     w = E.scenes.build_world(scene)
-    o = _make_oracle(O, scene)
+    o = P.oracle_for(O, scene)
     w.step(1000); o.step(1000)
     g, c = w.download_state(), o.state()
     rel = np.abs(g["pos"][0] - c["pos"][0]).max() / max(1.0, np.abs(c["pos"][0]).max())
@@ -226,7 +173,7 @@ def test_box_stacks_1000_steps(gpu, E, O):
     for the order-independent single-body case above."""
     scene = E.scenes.boxes_on_plane(3)
     w = E.scenes.build_world(scene)
-    o = _make_oracle(O, scene)
+    o = P.oracle_for(O, scene)
     w.step(1000); o.step(1000)
     g, c = w.download_state(), o.state()
     n = scene["dynamic"]
@@ -278,9 +225,9 @@ def test_full_size_mixed_pile_properties(gpu, E):
     for k in ("pos", "orn", "linvel", "angvel"):
         assert np.array_equal(st1[k], st2[k]), f"non-deterministic {k}"
     w1.run_phases(E.world.PH_BROAD)                 # bring the manifold set up to date with the moved AABBs ...
-    before = _pairset(w1.pairs(), ordered=False)
+    before = w1.pairs()
     w1.run_phases(E.world.PH_BROAD)                 # ... then a second pass over the same AABBs must change nothing
-    assert _pairset(w1.pairs(), ordered=False) == before, "broadphase is not idempotent on an unchanged state"
+    P.check_pairs("after a second broadphase", w1.pairs(), before)
     n = scene["dynamic"]
     assert st1["pos"][:n, 1].min() > -0.05, "bodies sank through the floor"
     assert s1["contact_points"] > n // 2

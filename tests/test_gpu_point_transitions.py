@@ -10,7 +10,7 @@ its manifold; a box hops on a box resting on a kinematic platform, so that its m
 while the island keeps its tile through the other manifold.
 
 Every step, in three modes (plain launches, CUDA graphs that skip the rebuild while graph_changed is clear, dataflow only):
-the oracle lock step of tests/emu/lockstep.py, the packing against its restatement (tests/tile_packing.py; in the graph
+the oracle lock step of tests/parity.py, the packing against its restatement (tests/tile_packing.py; in the graph
 mode a skipped rebuild whose inputs changed fails there), and the modes bit-identical to each other.  Also, with the
 step split after the narrowphase, graph_changed must be set on every step where one of those transitions happened: the
 CPU emulation has no CUDA graphs, and that check is what it can see of a missing flag."""
@@ -21,7 +21,7 @@ import numpy as np
 import pytest
 
 from tests import tile_packing as TP
-from tests.emu.lockstep import build_world, lockstep
+from tests.parity import build_world, lockstep, same_digests
 from tests.test_gpu_tile_edges import _Scene
 
 pytestmark = pytest.mark.gpu
@@ -129,9 +129,7 @@ def test_point_transitions_lockstep(gpu, E, O):
         if mode == "dataflow":
             assert tr.pc.tiled_steps == 0 and tr.seen["tile-less change"] > 0, tr.seen
         digests[mode] = res["digests"]
-    for mode in MODES[1:]:
-        diff = [s for s, (a, b) in enumerate(zip(digests[MODES[0]], digests[mode])) if a != b]
-        assert not diff, f"{mode} differs from {MODES[0]} from step {diff[0]} on"
+    same_digests(digests)
 
 
 def _counters(w):

@@ -12,7 +12,7 @@ import numpy as np
 import pytest
 
 from tests import tile_packing as TP
-from tests.emu.lockstep import lockstep
+from tests.parity import lockstep, same_digests
 from tests.test_ref_stepper import random_scene, random_scene_wide
 
 pytestmark = pytest.mark.gpu
@@ -36,10 +36,8 @@ def _all_modes(E, O, scene, steps, min_exact=None, **kw):
         assert pc.rebuilt + pc.reused == steps
         if mode == "dataflow":
             assert pc.tiled_steps == 0
-        digests[mode] = res["digests"]
-    for mode in MODES[1:]:
-        diff = [s for s, (a, b) in enumerate(zip(digests[MODES[0]], digests[mode])) if a != b]
-        assert not diff, f"{scene['name']}: {mode} differs from {MODES[0]} from step {diff[0]} on"
+        digests[f"{scene['name']} {mode}"] = res["digests"]
+    same_digests(digests)
     return checks["plain"]
 
 

@@ -14,6 +14,7 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 from tests import raycast_support as S  # noqa: E402
 from tests.emu import raycast as R  # noqa: E402
+from tests.parity import build_world, same_state  # noqa: E402
 
 
 def _bounds(st, kind):
@@ -113,18 +114,12 @@ def test_device_pointer_path_equals_host_path(gpu, E):
     assert (host["body"] != E.RAY_MISS).sum() > 1000
 
 
-def _world(E, scene, monkeypatch, graph, reuse=True):
-    with monkeypatch.context() as m:
-        m.setenv("B2D_GRAPH", "1" if graph else "0")
-        m.setenv("B2D_GRAPH_REUSE", "1" if reuse else "0")
-        return E.scenes.build_world(scene)
-
-
 @pytest.mark.parametrize("graph,reuse", [(True, True), (True, False), (False, True)])
-def test_raycasts_do_not_change_stepping(gpu, E, monkeypatch, graph, reuse):
+def test_raycasts_do_not_change_stepping(gpu, E, graph, reuse):
     """200 steps with a raycast batch after every step == 200 steps without: state bits and rebuild counters."""
     scene = E.scenes.hinge_chains(16, 16, 4)
-    quiet, busy = _world(E, scene, monkeypatch, graph, reuse), _world(E, scene, monkeypatch, graph, reuse)
+    env = dict(B2D_GRAPH="1" if graph else "0", B2D_GRAPH_REUSE="1" if reuse else "0")
+    quiet, busy = build_world(E, scene, env=env), build_world(E, scene, env=env)
     busy.step(1)
     quiet.step(1)
     lo, hi = _bounds(busy.download_state(), scene["bodies"]["kind"])
@@ -140,9 +135,7 @@ def test_raycasts_do_not_change_stepping(gpu, E, monkeypatch, graph, reuse):
             for w in (quiet, busy):
                 w.upload_bodies(ids, linvel=up)
     assert hits > 0
-    a, b = quiet.download_state(), busy.download_state()
-    for k in ("pos", "orn", "linvel", "angvel", "aabb"):
-        assert np.array_equal(a[k], b[k]), k
+    same_state(quiet, busy)
     sa, sb = quiet.stats(), busy.stats()
     assert (sa["steps_rebuilt"], sa["steps_reused"]) == (sb["steps_rebuilt"], sb["steps_reused"])
     assert sb["error_flags"] == 0

@@ -7,6 +7,8 @@ import os
 import numpy as np
 import pytest
 
+from tests.parity import build_world, same_state
+
 pytestmark = pytest.mark.gpu
 
 TIP_DEG = 40.0          # the tipping box stands on one edge, off balance: 2 contact points until it lands on a face
@@ -30,38 +32,24 @@ def _scene(E):
     return scene, len(b["kind"]) + 9
 
 
-def _world(E, scene, monkeypatch, graph, tiles=True):
-    with monkeypatch.context() as m:
-        m.setenv("B2D_GRAPH", "1" if graph else "0")
-        m.setenv("B2D_GRAPH_REUSE", "1")
-        m.setenv("B2D_TILES", "1" if tiles else "0")
-        return E.scenes.build_world(scene)
-
-
-def _same(a, b):
-    sa, sb = a.download_state(), b.download_state()
-    for k in ("pos", "orn", "linvel", "angvel", "aabb"):
-        assert np.array_equal(sa[k], sb[k]), k
-
-
 def _points(w, body):
     c = w.contacts()
     hit = np.nonzero((c["pairs"] == body).any(axis=1))[0]
     return int(c["num"][hit].max()) if len(hit) else 0
 
 
-def test_two_point_tile_crossing(gpu, E, monkeypatch):
+def test_two_point_tile_crossing(gpu, E):
     scene, box = _scene(E)
-    reuse = _world(E, scene, monkeypatch, graph=True)
-    plain = _world(E, scene, monkeypatch, graph=False)
-    dataflow = _world(E, scene, monkeypatch, graph=True, tiles=False)
+    reuse = build_world(E, scene, "graph")
+    plain = build_world(E, scene, "plain")
+    dataflow = build_world(E, scene, "graph", env=dict(B2D_TILES="0"))
     worlds = (reuse, plain, dataflow)
     crossing, history = None, []
     for step in range(150):
         r0 = reuse.stats()["steps_rebuilt"]
         for w in worlds:
             w.step(1)
-        _same(reuse, plain); _same(reuse, dataflow)
+        same_state(reuse, plain, dataflow)
         n = _points(reuse, box)
         rebuilt = reuse.stats()["steps_rebuilt"] - r0
         if crossing is None and history and 0 < history[-1][0] <= 2 < n:

@@ -8,7 +8,7 @@ generic islands in root order.
 
 Every step of every scene, in three modes (plain launches, CUDA graphs with rebuild reuse, dataflow only) and at three
 iteration settings ((1, 0): the tile kernel without position iterations): the packing against the restatement, the oracle lock step of
-tests/emu/lockstep.py, and the three modes bit-identical to each other.  Also runs against the CPU emulation
+tests/parity.py, and the three modes bit-identical to each other.  Also runs against the CPU emulation
 (B2D_EMU=1), which has no graphs and runs fewer steps."""
 import os
 
@@ -16,7 +16,7 @@ import numpy as np
 import pytest
 
 from tests import tile_packing as TP
-from tests.emu.lockstep import lockstep
+from tests.parity import lockstep, same_digests
 
 pytestmark = pytest.mark.gpu
 
@@ -183,6 +183,4 @@ def test_tile_edges_lockstep(gpu, E, O, name, iters):
         if mode == "dataflow":
             assert pc.tiled_steps == 0
         digests[mode] = res["digests"]
-    for mode in MODES[1:]:
-        diff = [s for s, (a, b) in enumerate(zip(digests[MODES[0]], digests[mode])) if a != b]
-        assert not diff, f"{mode} differs from {MODES[0]} from step {diff[0]} on"
+    same_digests(digests)

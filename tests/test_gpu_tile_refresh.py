@@ -11,7 +11,7 @@ import numpy as np
 import pytest
 
 from tests import tile_packing as TP
-from tests.emu.lockstep import build_world
+from tests.parity import build_world
 from tests.test_gpu_tile_edges import SCENES
 from tests.test_ref_stepper import random_scene
 

@@ -105,7 +105,7 @@ def test_device_chains_follow_the_real_stepper_free_running(gpu, E, O):
 def test_device_restitution_solver_matches_oracle(gpu, E, O):
     """B2D_FLAG_RESTITUTION_SOLVER on the device in lock step with the oracle's restatement of restitution_solver.cpp (the
     reference's default settings), mixed pile with e = 0.2 and a random scene with e up to 0.8."""
-    from tests.emu.lockstep import lockstep
+    from tests.parity import lockstep
     from tests.test_ref_stepper import random_scene
     for scene in (E.scenes.mixed_pile(5, jitter=0.01), random_scene(E, O, 3)):
         res = lockstep(E, O, scene, 100, restitution_solver=True)

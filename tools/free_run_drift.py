@@ -6,20 +6,15 @@ import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import edyn_b200 as E
 from oracle import oracle as O
+from tests import parity as P
 kind, n = sys.argv[1], int(sys.argv[2])
 scene = E.scenes.boxes_on_plane(n) if kind == "boxes" else E.scenes.hinge_chains(n, n)
 w = E.scenes.build_world(scene, max_manifolds=8 * len(scene["bodies"]["kind"]))
-o = O.OracleWorld(vel_iters=scene["settings"]["velocity_iterations"], pos_iters=scene["settings"]["position_iterations"], threads=os.cpu_count())
-o.add_bodies(scene["bodies"])
-if scene["hinges"]:
-    h = scene["hinges"]; o.add_hinges(h["a"], h["b"], h["pivot_a"], h["pivot_b"], h["axis_a"], h["axis_b"])
-if scene["exclusions"] is not None:
-    o.add_exclusions(*scene["exclusions"])
+o = P.oracle_for(O, scene, threads=os.cpu_count())
 nd = scene["dynamic"]
 for s in range(1000):
     w.run_phases(E.world.PH_ALL)
-    hi, pr = w.solver_order()
-    o.run_phases(O.PH_BROAD | O.PH_NARROW | O.PH_ISLANDS); o.set_order(hi, pr); o.run_phases(O.PH_SOLVE)
+    P.oracle_step(O, o, w)
     if s % 50 == 49:
         g, c = w.download_state(aabb=False), o.state()
         err = np.abs(g["pos"][:nd] - c["pos"][:nd]).max(axis=1)
