@@ -10,6 +10,7 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <map>
 #include <string>
 #include <unordered_set>
 #include <vector>
@@ -45,6 +46,7 @@ struct b2d_world {
     std::vector<uint32_t> large;
     std::vector<uint64_t> exclusions;
     uint32_t xhash_capacity = 0, xhash_used = 0;      // device exclusion table: slots, keys inserted (stale ones included)
+    std::map<uint32_t, float2> mixing;                // material_mix_table: material_pair_key -> (friction, restitution)
     bool contacts_dirty = false;
     uint64_t updates = 0;             // island updates so far (sleep timestamps)
     // broadphase classes: bounding diameter and kind per body (host mirror), re-derived lazily before the next step
@@ -108,6 +110,17 @@ static bool dalloc(b2d_world *w, T *&p, size_t n, int fill = 0) {
     p = static_cast<T *>(q);
     return true;
 }
+// The mixing table starts with room for MIX_SLOTS / 2 entries; edits that fit are uploaded in place, so captured step
+// graphs (which hold the table's pointers) stay valid.
+constexpr uint32_t MIX_SLOTS = 256;
+static void dfree(b2d_world *w, void *p) {
+    auto it = std::find(w->allocs.begin(), w->allocs.end(), p);
+    if (it != w->allocs.end()) { cudaFree(*it); w->allocs.erase(it); }
+}
+static uint32_t hash64_host(unsigned long long k) {      // hash64 of b2d_kernels.cuh
+    k ^= k >> 33; k *= 0xff51afd7ed558ccdULL; k ^= k >> 33; k *= 0xc4ceb9fe1a85ec53ULL; k ^= k >> 33;
+    return (uint32_t)k;
+}
 static uint32_t pow2_at_least(uint64_t v) { uint32_t p = 1; while (p < v) p <<= 1; return p; }
 static int blocks_for(b2d_world *w, uint64_t n, int threads) {
     uint64_t b = (n + threads - 1) / threads;
@@ -153,6 +166,9 @@ b2d_world *b2d_create(const b2d_config *cfg) {
     for (int k = 0; k < 3; ++k) { d.cell_org[k] = -(1 << 15); d.cell_bits[k] = 16; }
     bool ok = true;
     ok = ok && dalloc(w, d.pos, NB) && dalloc(w, d.orn, NB) && dalloc(w, d.linvel, NB) && dalloc(w, d.angvel, NB);
+    ok = ok && dalloc(w, d.matid, NB);
+    d.mix_size = MIX_SLOTS;
+    ok = ok && dalloc(w, d.mix_key, d.mix_size, 0xFF) && dalloc(w, d.mix_idx, d.mix_size) && dalloc(w, d.mix_mat, d.mix_size / 2);
     ok = ok && dalloc(w, d.dvw, 2 * (size_t)NB) && dalloc(w, d.invI, 3 * (size_t)NB) && dalloc(w, d.invIW, 3 * (size_t)NB);
     ok = ok && dalloc(w, d.grav, NB) && dalloc(w, d.shp, NB) && dalloc(w, d.bbmin, NB) && dalloc(w, d.bbmax, NB);
     ok = ok && dalloc(w, d.flags, NB) && dalloc(w, d.mat, NB) && dalloc(w, d.group, NB) && dalloc(w, d.fmask, NB);
@@ -342,9 +358,12 @@ int b2d_add_bodies(b2d_world *w, const b2d_bodies *b, uint32_t *first_id) {
         }
         if (sk == B2D_SHAPE_PLANE && b->kind[i] != B2D_STATIC) { w->error = "b2d_add_bodies: plane shapes must be static"; return B2D_ERR_UNSUPPORTED; }
         if (b->kind[i] > B2D_STATIC) { w->error = "b2d_add_bodies: bad body kind"; return B2D_ERR_ARGUMENT; }
+        if (b->material && b->material[i] > B2D_MATERIAL_UNASSIGNED && b->material[i] != B2D_MATERIAL_NONE) {
+            w->error = "b2d_add_bodies: material must be an id up to 0xFFFF or B2D_MATERIAL_NONE"; return B2D_ERR_ARGUMENT;
+        }
     }
     std::vector<float4> pos(n), orn(n), lv(n), av(n), invI(3 * (size_t)n), grav(n), shp(n);
-    std::vector<uint32_t> flags(n); std::vector<float2> mat(n); std::vector<unsigned long long> grp(n), msk(n);
+    std::vector<uint32_t> flags(n), matid(n); std::vector<float2> mat(n); std::vector<unsigned long long> grp(n), msk(n);
     for (uint32_t i = 0; i < n; ++i) {
         const uint32_t kind = b->kind[i], sk = b->shape_kind[i];
         const bool dyn = kind == B2D_DYNAMIC;
@@ -359,6 +378,9 @@ int b2d_add_bodies(b2d_world *w, const b2d_bodies *b, uint32_t *first_id) {
         if (dyn && (sk == B2D_SHAPE_SPHERE || sk == B2D_SHAPE_CAPSULE)) f |= F_ROLLING;
         unsigned long long g = b->group ? b->group[i] : ~0ULL, m = b->mask ? b->mask[i] : ~0ULL;
         if (b->group && b->mask && !(g == ~0ULL && m == ~0ULL)) f |= F_FILTER;
+        const uint32_t mid = b->material ? b->material[i] : B2D_MATERIAL_UNASSIGNED;
+        if (mid == B2D_MATERIAL_NONE) f |= F_SENSOR;
+        matid[i] = mid == B2D_MATERIAL_NONE ? MATERIAL_UNASSIGNED : mid;
         class_add(w, sk != B2D_SHAPE_NONE ? shape_diameter(sk, b->shape_params + 4 * i) : 0.0f, dyn);
         flags[i] = f; mat[i] = make_float2(b->friction[i], b->restitution[i]); grp[i] = g; msk[i] = m;
     }
@@ -372,6 +394,7 @@ int b2d_add_bodies(b2d_world *w, const b2d_bodies *b, uint32_t *first_id) {
     CK(cudaMemcpyAsync(d.shp + first, shp.data(), n * sizeof(float4), cudaMemcpyHostToDevice, s));
     CK(cudaMemcpyAsync(d.flags + first, flags.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
     CK(cudaMemcpyAsync(d.mat + first, mat.data(), n * sizeof(float2), cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(d.matid + first, matid.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
     CK(cudaMemcpyAsync(d.group + first, grp.data(), n * sizeof(unsigned long long), cudaMemcpyHostToDevice, s));
     CK(cudaMemcpyAsync(d.fmask + first, msk.data(), n * sizeof(unsigned long long), cudaMemcpyHostToDevice, s));
     d.nbodies = first + n;
@@ -480,9 +503,8 @@ static int upload_exclusions(b2d_world *w) {
     Dev &d = w->d;
     uint32_t size = pow2_at_least(4ull * w->exclusions.size() + 1024);    // load <= 1/4: room for insert_exclusions
     std::vector<unsigned long long> table(size, ~0ULL);
-    auto h64 = [](unsigned long long k) { k ^= k >> 33; k *= 0xff51afd7ed558ccdULL; k ^= k >> 33; k *= 0xc4ceb9fe1a85ec53ULL; k ^= k >> 33; return (uint32_t)k; };
     for (uint64_t k : w->exclusions) {
-        uint32_t h = h64(k) & (size - 1);
+        uint32_t h = hash64_host(k) & (size - 1);
         while (table[h] != ~0ULL && table[h] != k) h = (h + 1) & (size - 1);
         table[h] = k;
     }
@@ -490,10 +512,7 @@ static int upload_exclusions(b2d_world *w) {
     if (!dalloc(w, dev, size)) return B2D_ERR_CUDA;
     CK(cudaMemcpyAsync(dev, table.data(), size * sizeof(unsigned long long), cudaMemcpyHostToDevice, w->stream));
     CK(cudaStreamSynchronize(w->stream));
-    if (d.xhash_key) {                                   // the table this one replaces
-        auto it = std::find(w->allocs.begin(), w->allocs.end(), (void *)d.xhash_key);
-        if (it != w->allocs.end()) { cudaFree(*it); w->allocs.erase(it); }
-    }
+    if (d.xhash_key) dfree(w, d.xhash_key);             // the table this one replaces
     d.xhash_key = dev; d.xhash_size = w->exclusions.empty() ? 0u : size;
     w->xhash_capacity = size; w->xhash_used = (uint32_t)w->exclusions.size();
     drop_graphs(w);
@@ -539,6 +558,65 @@ int b2d_remove_exclusions(b2d_world *w, uint32_t n, const uint32_t *a, const uin
     }
     w->exclusions.erase(std::remove_if(w->exclusions.begin(), w->exclusions.end(), [&](uint64_t k) { return gone.count(k) != 0; }), w->exclusions.end());
     return upload_exclusions(w);
+}
+
+// material_mix_table on the device: the whole table is re-hashed on the host and uploaded in place; only when it outgrows
+// its slots is it reallocated, which invalidates the captured step graphs.
+static int upload_mixing(b2d_world *w) {
+    Dev &d = w->d;
+    uint32_t size = d.mix_size;
+    while (2ull * w->mixing.size() > size) size *= 2;
+    std::vector<unsigned long long> keys(size, EMPTY_KEY);
+    std::vector<uint32_t> idx(size, 0);
+    std::vector<float2> mat(size / 2);
+    uint32_t k = 0;
+    for (const auto &e : w->mixing) {
+        uint32_t h = hash64_host(e.first) & (size - 1);
+        while (keys[h] != EMPTY_KEY) h = (h + 1) & (size - 1);
+        keys[h] = e.first; idx[h] = k; mat[k++] = e.second;
+    }
+    if (size != d.mix_size) {
+        CK(cudaStreamSynchronize(w->stream));
+        dfree(w, d.mix_key); dfree(w, d.mix_idx); dfree(w, d.mix_mat);
+        if (!dalloc(w, d.mix_key, size) || !dalloc(w, d.mix_idx, size) || !dalloc(w, d.mix_mat, size / 2)) return B2D_ERR_CUDA;
+        d.mix_size = size;
+        drop_graphs(w);
+    }
+    CK(cudaMemcpyAsync(d.mix_key, keys.data(), size * sizeof(unsigned long long), cudaMemcpyHostToDevice, w->stream));
+    CK(cudaMemcpyAsync(d.mix_idx, idx.data(), size * sizeof(uint32_t), cudaMemcpyHostToDevice, w->stream));
+    CK(cudaMemcpyAsync(d.mix_mat, mat.data(), (size / 2) * sizeof(float2), cudaMemcpyHostToDevice, w->stream));
+    CK(cudaStreamSynchronize(w->stream));
+    return B2D_OK;
+}
+static int mixing_ids_ok(b2d_world *w, uint32_t n, const uint32_t *id0, const uint32_t *id1, const char *fn) {
+    if (n && (!id0 || !id1)) { w->error = std::string(fn) + ": NULL id array"; return B2D_ERR_ARGUMENT; }
+    for (uint32_t k = 0; k < n; ++k)
+        if (id0[k] >= B2D_MATERIAL_UNASSIGNED || id1[k] >= B2D_MATERIAL_UNASSIGNED) {
+            w->error = std::string(fn) + ": material ids must be below 0xFFFF"; return B2D_ERR_ARGUMENT;
+        }
+    return B2D_OK;
+}
+static uint32_t mixing_key(uint32_t a, uint32_t b) { return a < b ? (a << 16) | b : (b << 16) | a; }     // material_pair_key
+
+int b2d_set_material_mixing(b2d_world *w, uint32_t n, const uint32_t *id0, const uint32_t *id1, const float *friction,
+                            const float *restitution) {
+    if (!w) return B2D_ERR_ARGUMENT;
+    if (int rc = mixing_ids_ok(w, n, id0, id1, "b2d_set_material_mixing")) return rc;
+    if (n && (!friction || !restitution)) { w->error = "b2d_set_material_mixing: NULL friction or restitution"; return B2D_ERR_ARGUMENT; }
+    if (!n) return B2D_OK;
+    cudaSetDevice(w->cfg.device);
+    for (uint32_t k = 0; k < n; ++k) w->mixing[mixing_key(id0[k], id1[k])] = make_float2(friction[k], restitution[k]);
+    return upload_mixing(w);
+}
+
+int b2d_remove_material_mixing(b2d_world *w, uint32_t n, const uint32_t *id0, const uint32_t *id1) {
+    if (!w) return B2D_ERR_ARGUMENT;
+    if (int rc = mixing_ids_ok(w, n, id0, id1, "b2d_remove_material_mixing")) return rc;
+    if (!n) return B2D_OK;
+    cudaSetDevice(w->cfg.device);
+    size_t erased = 0;
+    for (uint32_t k = 0; k < n; ++k) erased += w->mixing.erase(mixing_key(id0[k], id1[k]));
+    return erased ? upload_mixing(w) : B2D_OK;
 }
 
 // ------------------------------------------------------------------ one step
@@ -1319,8 +1397,20 @@ int b2d_upload_bodies(b2d_world *w, uint32_t n, const uint32_t *ids, const b2d_b
     for (uint32_t k = 0; k < n; ++k) {
         if (ids[k] >= d.nbodies) { w->error = "b2d_upload_bodies: body id out of range"; return B2D_ERR_ARGUMENT; }
         if (p->kind && p->kind[k] > B2D_STATIC) { w->error = "b2d_upload_bodies: bad body kind"; return B2D_ERR_ARGUMENT; }
+        if (p->material && p->material[k] > B2D_MATERIAL_UNASSIGNED && p->material[k] != B2D_MATERIAL_NONE) {
+            w->error = "b2d_upload_bodies: material must be an id up to 0xFFFF or B2D_MATERIAL_NONE"; return B2D_ERR_ARGUMENT;
+        }
     }
-    if ((size_t)n * 30 > w->stage_floats) { w->error = "b2d_upload_bodies: patch larger than the staging buffer"; return B2D_ERR_CAPACITY; }
+    if (p->material) {          // a body's points keep the constraint type they were created with: no sensor toggling
+        std::vector<uint32_t> flags(d.nbodies);
+        CK(cudaMemcpyAsync(flags.data(), d.flags, d.nbodies * sizeof(uint32_t), cudaMemcpyDeviceToHost, w->stream));
+        CK(cudaStreamSynchronize(w->stream));
+        for (uint32_t k = 0; k < n; ++k)
+            if (((flags[ids[k]] & F_SENSOR) != 0) != (p->material[k] == B2D_MATERIAL_NONE)) {
+                w->error = "b2d_upload_bodies: a body cannot change between sensor (B2D_MATERIAL_NONE) and material"; return B2D_ERR_UNSUPPORTED;
+            }
+    }
+    if ((size_t)n * 31 > w->stage_floats) { w->error = "b2d_upload_bodies: patch larger than the staging buffer"; return B2D_ERR_CAPACITY; }
     cudaStream_t s = w->stream;
     float *cur = w->stage;
     auto put = [&](const void *host, size_t words) -> const float * {
@@ -1334,6 +1424,7 @@ int b2d_upload_bodies(b2d_world *w, uint32_t n, const uint32_t *ids, const b2d_b
     q.pos = put(p->pos, 3 * (size_t)n); q.orn = put(p->orn, 4 * (size_t)n); q.linvel = put(p->linvel, 3 * (size_t)n); q.angvel = put(p->angvel, 3 * (size_t)n);
     q.inv_mass = put(p->inv_mass, n); q.inv_inertia = put(p->inv_inertia, 9 * (size_t)n); q.gravity = put(p->gravity, 3 * (size_t)n);
     q.friction = put(p->friction, n); q.restitution = put(p->restitution, n); q.kind = (const uint32_t *)put(p->kind, n);
+    q.material = (const uint32_t *)put(p->material, n);
     LAUNCH(k_patch_bodies, n, 256, d, dev_ids, n, q);
     if (p->kind) mark_graph_changed(w);              // body kinds decide the islands and which constraints have rows
     CK(cudaStreamSynchronize(s));                    // the host arrays may be reused by the caller

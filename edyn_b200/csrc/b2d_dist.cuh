@@ -60,6 +60,7 @@ __global__ void k_large_set(Dev d) { GRID_STRIDE(k, d.nlarge) d.flags[d.large_li
 struct Patch {      // device copies of the host arrays, nullptr = component untouched
     const float *pos, *orn, *linvel, *angvel, *inv_mass, *inv_inertia, *gravity, *friction, *restitution;
     const uint32_t *kind;
+    const uint32_t *material;       // material ids; the host has refused changes between sensor and non-sensor
 };
 // registry.patch / replace on a subset of bodies: only the named components change; AABB and inertia_world_inv follow
 // the transform the way solver.cpp:453-465 refreshes them.  A kind change re-derives what make_rigidbody sets per kind
@@ -89,6 +90,7 @@ __global__ void k_patch_bodies(Dev d, const uint32_t *ids, uint32_t n, Patch p) 
         if (p.friction) m.x = p.friction[k];
         if (p.restitution) m.y = p.restitution[k];
         d.mat[i] = m;
+        if (p.material && !(f & F_SENSOR)) d.matid[i] = p.material[k];
         f &= ~F_SLEEPING;                       // a patched body is awake (registry.patch wakes the island)
         d.flags[i] = f;
         const v3 pos = mk3(d.pos[i]); const q4 orn = mkq(d.orn[i]);
@@ -181,6 +183,7 @@ __global__ void k_plan_constraints(Dev d, uint32_t *counts) {
 
 // ---------------------------------------------------------------- hand-over blob
 // header (4 x uint4) | bodies: 11 float4 each | manifolds: 21 float4 each | hinges: 7 float4 each | exclusions: uint2 each
+// A body's flags carry F_SENSOR; its material id sits in o[10].z.
 constexpr uint32_t BLOB_MAGIC = 0xB2D0B10Bu;
 constexpr uint32_t BLOB_BODY_F4 = 11, BLOB_MANIFOLD_F4 = 21, BLOB_HINGE_F4 = 7;
 struct BlobHeader { uint32_t magic, nb, nm, nh, nx; uint32_t pad[11]; };      // 64 B
@@ -205,7 +208,7 @@ __global__ void k_pack_bodies(Dev d, const uint32_t *ids, uint32_t n, float4 *ou
         o[4] = d.invI[3 * (size_t)i]; o[5] = d.invI[3 * (size_t)i + 1]; o[6] = d.invI[3 * (size_t)i + 2];
         o[7] = g; o[8] = d.shp[i];
         o[9] = make_float4(m.x, m.y, fbits((uint32_t)grp), fbits((uint32_t)(grp >> 32)));
-        o[10] = make_float4(fbits((uint32_t)msk), fbits((uint32_t)(msk >> 32)), 0, 0);
+        o[10] = make_float4(fbits((uint32_t)msk), fbits((uint32_t)(msk >> 32)), fbits(d.matid[i]), 0);
     }
 }
 // flags for the deterministic compaction (slot order) of the constraints that leave for `dst`
@@ -272,6 +275,7 @@ __global__ void k_unpack_bodies(Dev d, uint32_t first, uint32_t n, const float4 
         d.mat[i] = make_float2(o[9].x, o[9].y);
         d.group[i] = (unsigned long long)ubits(o[9].z) | ((unsigned long long)ubits(o[9].w) << 32);
         d.fmask[i] = (unsigned long long)ubits(o[10].x) | ((unsigned long long)ubits(o[10].y) << 32);
+        d.matid[i] = ubits(o[10].z);
         d.flags[i] = f;
         ehash_insert(d.ehash, d.ehash_size, d.entity[i], i);
     }

@@ -67,6 +67,22 @@ B2D_D bool hash_find(const unsigned long long *keys, const uint32_t *vals, uint3
     }
 }
 
+// a manifold with a sensor on either side has points but no rows and no restitution
+B2D_D bool sensor_pair(uint32_t fa, uint32_t fb) { return ((fa | fb) & F_SENSOR) != 0u; }
+B2D_D unsigned long long material_pair_key(uint32_t ia, uint32_t ib) { return ia < ib ? ((unsigned long long)ia << 16) | ib : ((unsigned long long)ib << 16) | ia; }
+// friction and restitution of a new contact point between bodies a and b (collision_util.cpp:282-317): the mixing table's
+// entry for their two material ids, else the mix of dynamics/material_mixing.hpp:12-18.  A sensor's points have no
+// contact_point_material: (0, 0).
+B2D_D float2 pair_material(const Dev &d, uint32_t a, uint32_t b) {
+    if (sensor_pair(d.flags[a], d.flags[b])) return make_float2(0.0f, 0.0f);
+    const uint32_t ia = d.matid[a], ib = d.matid[b];
+    uint32_t k;
+    if (ia != MATERIAL_UNASSIGNED && ib != MATERIAL_UNASSIGNED && hash_find(d.mix_key, d.mix_idx, d.mix_size, material_pair_key(ia, ib), k))
+        return d.mix_mat[k];
+    const float2 A = d.mat[a], B = d.mat[b];
+    return make_float2(sqrtf(A.x * B.x), fminf(A.y, B.y));
+}
+
 B2D_D box3 body_box(const Dev &d, uint32_t i) { box3 b; b.mn = mk3(d.bbmin[i]); b.mx = mk3(d.bbmax[i]); return b; }
 B2D_D m3 load_m3(const float4 *p, uint32_t i) { m3 m; m.r0 = mk3(p[3 * i]); m.r1 = mk3(p[3 * i + 1]); m.r2 = mk3(p[3 * i + 2]); return m; }
 B2D_D void store_invIW(const Dev &d, uint32_t i, const m3 &m, float inv_m) {
@@ -537,14 +553,14 @@ B2D_D void merge_point(const CPoint &rp, MPoint &cp, q4 ornA, q4 ornB) {
     if (rp.att != ATT_NONE) cp.local_normal = rotate(conjugate(rp.att == ATT_A ? ornA : ornB), rp.normal);
     else cp.local_normal = mk3(0, 0, 0);
 }
-// create_contact_point, collision_util.cpp:319-395; mixing dynamics/material_mixing.hpp:12-18
-B2D_D MPoint create_point(const CPoint &rp, q4 ornA, q4 ornB, float2 matA, float2 matB) {
+// create_contact_point, collision_util.cpp:319-395; mat = pair_material of the two bodies
+B2D_D MPoint create_point(const CPoint &rp, q4 ornA, q4 ornB, float2 mat) {
     MPoint cp;
     cp.pivotA = rp.pivotA; cp.pivotB = rp.pivotB; cp.normal = rp.normal; cp.att = rp.att; cp.distance = rp.distance;
     if (rp.att != ATT_NONE) cp.local_normal = rotate(conjugate(rp.att == ATT_A ? ornA : ornB), rp.normal);
     else cp.local_normal = mk3(0, 0, 0);
-    cp.friction = sqrtf(matA.x * matB.x);
-    cp.restitution = fminf(matA.y, matB.y);
+    cp.friction = mat.x;
+    cp.restitution = mat.y;
     cp.lifetime = 0;
     return cp;
 }
@@ -681,13 +697,13 @@ B2D_D int np_rearrange(const Dev &d, uint32_t m, uint2 pr, const CResult &res, u
     #pragma unroll 1
     for (int j = 0; j < num; ++j) place(j, false);
     if (created) {
-        const float2 matA = d.mat[pr.x], matB = d.mat[pr.y];
+        const float2 mat = pair_material(d, pr.x, pr.y);
         const q4 ornA = mkq(d.orn[pr.x]), ornB = mkq(d.orn[pr.y]);
         int dst = n_created;
         #pragma unroll 1
         for (int j = 0; j < num_points; ++j) {
             if (!(created >> j & 1u)) continue;
-            store_point(d, m, --dst, create_point(res.pt[lsrc >> 2 * j & 3u], ornA, ornB, matA, matB));
+            store_point(d, m, --dst, create_point(res.pt[lsrc >> 2 * j & 3u], ornA, ornB, mat));
             d.pI[(size_t)dst * d.NM + m] = make_float4(0, 0, 0, 0);
         }
     }
@@ -957,8 +973,11 @@ __global__ void k_color_list(Dev d, int recolor) {
             if (!(st & MS_NPTS_MASK)) continue;
         }
         const uint2 p = d.mpair[m];
-        const bool da = is_dynamic(d.flags[p.x]), db = is_dynamic(d.flags[p.y]);
-        if (!da && !db) {          // sleeping: drops its colour, takes a fresh one when the island wakes
+        const uint32_t fa = d.flags[p.x], fb = d.flags[p.y];
+        const bool da = is_dynamic(fa), db = is_dynamic(fb);
+        // sleeping: drops its colour, takes a fresh one when the island wakes.  A sensor's manifold never has rows: the
+        // single point where a manifold enters the solver (colour, tile census, sort key) is here
+        if ((!da && !db) || sensor_pair(fa, fb)) {
             if (col != COLOR_NONE) d.mstate[m] = st | MS_COLOR_MASK;
             continue;
         }
@@ -2530,7 +2549,7 @@ __global__ void k_rest_solve(Dev d) {
                     if (e >> 31) {
                         const uint32_t m = d.radj_m[o + k];
                         const uint2 pr = d.mpair[m];
-                        if (fminf(d.mat[pr.x].y, d.mat[pr.y].y) > EPS) {            // contact_manifold_with_restitution, constraint_util.cpp:86-101
+                        if (pair_material(d, pr.x, pr.y).y > EPS) {                  // contact_manifold_with_restitution, constraint_util.cpp:86-101
                             const float rel = rest_min_relvel(d, m);
                             const unsigned long long key = pair_key(pr.x, pr.y);
                             if (rel < best || (rel == best && best_m != NONE && key < best_key)) { best = rel; best_m = m; best_key = key; }
@@ -2562,6 +2581,9 @@ __global__ void k_rest_solve(Dev d) {
                 for (uint32_t k = 0; k < n; ++k) {
                     if (!(d.radj[o + k] >> 31)) continue;
                     const uint32_t m = d.radj_m[o + k];
+                    const uint2 pr = d.mpair[m];
+                    // a sensor's manifold stays an edge of the walk but is never solved: its points have no material
+                    if (sensor_pair(d.flags[pr.x], d.flags[pr.y])) continue;
                     if (rest_min_relvel(d, m) < threshold) {
                         if (ng == REST_MAX_MANIFOLDS) { atomicOr(&d.cnt->err, ERR_RESTITUTION_GROUP); break; }
                         group[ng++] = m;

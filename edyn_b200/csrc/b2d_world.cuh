@@ -11,10 +11,13 @@ namespace b2d {
 constexpr uint32_t F_KIND_MASK = 3u;          // 0 dynamic, 1 kinematic, 2 static (B2D_DYNAMIC..)
 constexpr uint32_t F_SHAPE_SHIFT = 4;         // bits 4..11 shape kind
 constexpr uint32_t F_ROLLING = 1u << 12;      // rolling_tag (util/rigidbody.cpp:120-130)
+constexpr uint32_t F_SENSOR = 1u << 17;       // no material component: its manifolds get points but no rows (collision_util.cpp:358-384)
 constexpr uint32_t F_FILTER = 1u << 13;       // has collision_filter
 constexpr uint32_t F_LARGE = 1u << 14;        // larger than a broadphase cell: brute-force list
 constexpr uint32_t F_SLEEPING = 1u << 16;     // sleeping_tag: excluded from every per-step view until its island wakes
 constexpr uint32_t F_REMOVED = 1u << 15;      // destroyed (b2d_remove_bodies): static, shapeless, its manifolds and joints die
+
+constexpr uint32_t MATERIAL_UNASSIGNED = 0xFFFFu;   // material::UnassignedID: never in the mixing table
 
 // mstate word per manifold slot
 constexpr uint32_t MS_NPTS_MASK = 7u;
@@ -192,6 +195,11 @@ struct Dev {
     // ---- narrowphase: manifold slots sorted by pair type (its own buffer: cidx_s, the solver order, outlives a step
     // whose island rebuild is skipped)
     uint32_t *npidx;
+
+    // ---- materials: material::id per body (MATERIAL_UNASSIGNED = no id), and the material_mix_table as an open-addressing
+    // hash of the unordered id pair (lo << 16 | hi) -> index into mix_mat (friction, restitution); mix_size slots
+    uint32_t *matid;
+    unsigned long long *mix_key; uint32_t *mix_idx; float2 *mix_mat; uint32_t mix_size;
 };
 
 } // namespace b2d

@@ -36,7 +36,9 @@ struct box_shape { vector3 half_extents; };
 struct plane_shape { vector3 normal; scalar constant; };
 using shapes_variant_t = std::variant<sphere_shape, capsule_shape, box_shape, plane_shape>;
 
-struct material { scalar restitution{0}; scalar friction{0.5f}; };
+struct material_base { scalar restitution{0}; scalar friction{0.5f}; };
+// material::id keys the mixing table (insert_material_mixing); UnassignedID never matches an entry
+struct material : material_base { using id_type = std::uint16_t; static constexpr id_type UnassignedID = 0xFFFF; id_type id{UnassignedID}; };
 enum class rigidbody_kind : std::uint8_t { rb_dynamic, rb_kinematic, rb_static };
 
 struct rigidbody_def {                               // include/edyn/util/rigidbody.hpp
@@ -155,7 +157,8 @@ inline entity make_rigidbody(registry &r, const rigidbody_def &def) {
     float grav[3] = {g.x, g.y, g.z};
     float fr = def.material ? def.material->friction : 0, re = def.material ? def.material->restitution : 0;
     std::uint64_t grp = def.collision_group, msk = def.collision_mask;
-    b2d_bodies b{1, pos, orn, lv, av, &inv_mass, inv_I.data(), grav, &kind, &sk, sp, &fr, &re, &grp, &msk};
+    std::uint32_t mat = def.material ? std::uint32_t(def.material->id) : B2D_MATERIAL_NONE;      // no material: a sensor
+    b2d_bodies b{1, pos, orn, lv, av, &inv_mass, inv_I.data(), grav, &kind, &sk, sp, &fr, &re, &grp, &msk, &mat};
     std::uint32_t id = 0;
     detail::check(r, b2d_add_bodies(r.world, &b, &id), "b2d_add_bodies");
     r.position.insert(r.position.end(), pos, pos + 3); r.orientation.insert(r.orientation.end(), orn, orn + 4);
@@ -168,6 +171,12 @@ inline void make_hinge(registry &r, entity a, entity b, vector3 pivot_a, vector3
     float pa[3] = {pivot_a.x, pivot_a.y, pivot_a.z}, pb[3] = {pivot_b.x, pivot_b.y, pivot_b.z};
     float xa[3] = {axis_a.x, axis_a.y, axis_a.z}, xb[3] = {axis_b.x, axis_b.y, axis_b.z};
     detail::check(r, b2d_add_hinges(r.world, 1, &a, &b, pa, pb, xa, xb), "b2d_add_hinges");
+}
+// edyn::insert_material_mixing (util/insert_material_mixing.cpp:9-22): contact points created from now on between bodies of
+// material ids id0 and id1 (either order) take this friction and restitution instead of the mixed ones
+inline void insert_material_mixing(registry &r, material::id_type id0, material::id_type id1, const material_base &m) {
+    std::uint32_t a = id0, b = id1; float f = m.friction, e = m.restitution;
+    detail::check(r, b2d_set_material_mixing(r.world, 1, &a, &b, &f, &e), "b2d_set_material_mixing");
 }
 inline void exclude_collision(registry &r, entity a, entity b) { detail::check(r, b2d_add_exclusions(r.world, 1, &a, &b), "b2d_add_exclusions"); }
 

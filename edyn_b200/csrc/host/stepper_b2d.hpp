@@ -27,6 +27,7 @@
 #include <edyn/comp/tag.hpp>
 #include <edyn/constraints/hinge_constraint.hpp>
 #include <edyn/context/settings.hpp>
+#include <edyn/dynamics/material_mixing.hpp>
 #include <edyn/shapes/shapes.hpp>
 #include <edyn/util/visit_component.hpp>
 #include "b2d.h"
@@ -34,9 +35,19 @@
 #include <cstdint>
 #include <stdexcept>
 #include <string>
+#include <map>
+#include <set>
 #include <unordered_map>
 #include <utility>
 #include <vector>
+
+// The mixing-table entry points are referenced weakly: this header-only binding also loads against a libb2d built before
+// they existed, and then refuses a registry whose material_mix_table holds entries (sync_material_table).
+extern "C" {
+int b2d_set_material_mixing(b2d_world *w, uint32_t n, const uint32_t *id0, const uint32_t *id1, const float *friction,
+                            const float *restitution) __attribute__((weak));
+int b2d_remove_material_mixing(b2d_world *w, uint32_t n, const uint32_t *id0, const uint32_t *id1) __attribute__((weak));
+}
 
 namespace edyn {
 
@@ -56,6 +67,10 @@ class stepper_b2d {
     std::vector<entt::entity> m_dirty, m_exclusion_dirty;    // entities the user patched since the last step
     std::vector<std::vector<uint32_t>> m_excluded;           // body id -> ids it is staged as excluded from
     std::vector<uint8_t> m_is_dirty;
+    std::vector<uint8_t> m_sensor;                           // body id -> staged without a material (B2D_MATERIAL_NONE)
+    std::vector<entt::entity> m_material_toggled;            // material emplaced on / removed from an entity since the last step
+    std::set<uint32_t> m_material_ids;                       // material::id values staged so far (UnassignedID excluded)
+    std::map<uint32_t, std::pair<float, float>> m_mixing;    // the material_mix_table entries staged: lo << 16 | hi -> (friction, restitution)
     std::vector<uint32_t> m_asleep, m_was_asleep;            // B2D_FLAG_SLEEPING: sleeping_tag per body, this step / last step
     bool m_sleeping {false};
     std::vector<float> m_pos, m_orn, m_lv, m_av, m_aabb;     // download buffers
@@ -107,6 +122,8 @@ public:
         registry.on_update<inertia_inv>().connect<&stepper_b2d::on_update_body>(*this);
         registry.on_update<gravity>().connect<&stepper_b2d::on_update_body>(*this);
         registry.on_update<material>().connect<&stepper_b2d::on_update_body>(*this);
+        registry.on_construct<material>().connect<&stepper_b2d::on_material_toggled>(*this);
+        registry.on_destroy<material>().connect<&stepper_b2d::on_material_toggled>(*this);
         for (auto e : registry.view<rigidbody_tag>()) m_new_bodies.push_back(e);       // bodies that predate the stepper,
         std::reverse(m_new_bodies.begin(), m_new_bodies.end());                        // oldest first (views go newest first)
         for (auto e : registry.view<hinge_constraint>()) m_new_hinges.push_back(e);
@@ -130,6 +147,8 @@ public:
         r.on_update<inertia_inv>().disconnect<&stepper_b2d::on_update_body>(*this);
         r.on_update<gravity>().disconnect<&stepper_b2d::on_update_body>(*this);
         r.on_update<material>().disconnect<&stepper_b2d::on_update_body>(*this);
+        r.on_construct<material>().disconnect<&stepper_b2d::on_material_toggled>(*this);
+        r.on_destroy<material>().disconnect<&stepper_b2d::on_material_toggled>(*this);
         b2d_destroy(m_world);
     }
 
@@ -158,6 +177,8 @@ public:
         m_dirty.push_back(e);
     }
     void on_exclusion_changed(entt::registry &, entt::entity e) { m_exclusion_dirty.push_back(e); }
+    // checked at the next step (registry.destroy(body) removes the material too, which is no toggle)
+    void on_material_toggled(entt::registry &, entt::entity e) { if (id_of(e) != no_id) m_material_toggled.push_back(e); }
 
     // ---- staging: registry -> device
     void stage_new_bodies() {                                          // make_rigidbody's components -> b2d_bodies (SoA)
@@ -168,6 +189,7 @@ public:
         std::vector<float> pos(3 * n), orn(4 * n), lv(3 * n), av(3 * n), im(n), iI(9 * n), g(3 * n), sp(4 * n), fr(n), re(n);
         std::vector<uint32_t> kind(n), sk(n);
         std::vector<uint64_t> grp(n, ~0ull), msk(n, ~0ull);
+        std::vector<uint32_t> mid(n, B2D_MATERIAL_NONE);                    // no material component: a sensor
         for (uint32_t i = 0; i < n; ++i) {
             const auto e = m_new_bodies[i];
             put3(&pos[3 * i], reg.get<position>(e));
@@ -181,7 +203,10 @@ public:
                 for (int r = 0; r < 3; ++r) put3(&iI[9 * i + 3 * r], I.row[r]);
                 if (auto *gr = reg.try_get<gravity>(e)) put3(&g[3 * i], *gr);
             }
-            if (auto *m = reg.try_get<material>(e)) { fr[i] = float(m->friction); re[i] = float(m->restitution); }
+            if (auto *m = reg.try_get<material>(e)) {
+                fr[i] = float(m->friction); re[i] = float(m->restitution); mid[i] = m->id;
+                if (m->id != material::UnassignedID) m_material_ids.insert(m->id);
+            }
             sk[i] = B2D_SHAPE_NONE;
             if (auto *si = reg.try_get<shape_index>(e)) {
                 sk[i] = uint32_t(si->value);                                   // shapes.hpp:23-37 order == B2D_SHAPE_* values
@@ -195,7 +220,7 @@ public:
             if (auto *f = reg.try_get<collision_filter>(e)) { grp[i] = f->group; msk[i] = f->mask; }
         }
         b2d_bodies b {n, pos.data(), orn.data(), lv.data(), av.data(), im.data(), iI.data(), g.data(), kind.data(), sk.data(), sp.data(),
-                      fr.data(), re.data(), grp.data(), msk.data()};
+                      fr.data(), re.data(), grp.data(), msk.data(), mid.data()};
         uint32_t first = 0;
         check(b2d_add_bodies(m_world, &b, &first), "b2d_add_bodies");
         for (uint32_t i = 0; i < n; ++i) {
@@ -208,6 +233,7 @@ public:
         }
         m_excluded.resize(m_entities.size());
         m_is_dirty.resize(m_entities.size(), 0);
+        for (uint32_t i = 0; i < n; ++i) m_sensor.push_back(mid[i] == B2D_MATERIAL_NONE ? 1 : 0);
         m_new_bodies.clear();
     }
 
@@ -270,6 +296,7 @@ public:
         auto &reg = *m_registry;
         std::vector<uint32_t> ids;
         std::vector<float> pos, orn, lv, av, im, iI, g, fr, re;
+        std::vector<uint32_t> mid;
         for (auto e : m_dirty) {
             const uint32_t id = reg.valid(e) ? id_of(e) : no_id;
             if (id == no_id) continue;
@@ -290,11 +317,60 @@ public:
             put3(t, gr ? vector3(*gr) : vector3_zero); g.insert(g.end(), t, t + 3);
             auto *m = reg.try_get<material>(e);
             fr.push_back(m ? float(m->friction) : 0.f); re.push_back(m ? float(m->restitution) : 0.f);
+            mid.push_back(m ? uint32_t(m->id) : B2D_MATERIAL_NONE);
+            if (m && m->id != material::UnassignedID) m_material_ids.insert(m->id);
         }
         m_dirty.clear();
         if (ids.empty()) return;
-        b2d_body_patch p {pos.data(), orn.data(), lv.data(), av.data(), im.data(), iI.data(), g.data(), fr.data(), re.data(), nullptr};
+        b2d_body_patch p {pos.data(), orn.data(), lv.data(), av.data(), im.data(), iI.data(), g.data(), fr.data(), re.data(), nullptr, mid.data()};
         check(b2d_upload_bodies(m_world, uint32_t(ids.size()), ids.data(), &p), "b2d_upload_bodies");
+    }
+
+    // A staged body cannot gain or lose its material: the device fixes a point's constraint type (contact_constraint or
+    // null_constraint) when the point is created, as the reference does, and does not track it per point.
+    void check_material_toggles() {
+        auto &reg = *m_registry;
+        for (auto e : m_material_toggled) {
+            const uint32_t id = reg.valid(e) ? id_of(e) : no_id;
+            if (id != no_id && reg.all_of<material>(e) == (m_sensor[id] != 0))
+                throw std::runtime_error("stepper_b2d: emplacing or removing the material of an existing body (sensor <-> non-sensor) is not supported");
+        }
+        m_material_toggled.clear();
+    }
+
+    // material_mix_table (dynamics/material_mixing.hpp:36-80) has no iteration API and raises no signal: every step probes
+    // try_get for each unordered pair of the material ids staged so far (k (k + 1) / 2 pairs for k ids, each looked up in
+    // both orders when the first misses), and uploads what
+    // changed since the last step.  Entries with contact extras (spin / roll friction, stiffness / damping) are out of scope.
+    void sync_material_table() {
+        auto *table = m_registry->ctx().find<material_mix_table>();
+        if (!table || m_material_ids.empty()) return;
+        std::vector<uint32_t> set_a, set_b, del_a, del_b;
+        std::vector<float> set_f, set_r;
+        for (auto i = m_material_ids.begin(); i != m_material_ids.end(); ++i) {
+            for (auto j = i; j != m_material_ids.end(); ++j) {
+                const uint32_t key = (*i << 16) | *j;
+                // both orders: unordered_pair's operator< (core/unordered_pair.hpp) is no strict weak ordering, so the
+                // std::map can miss an entry inserted as (j, i) when it is looked up as (i, j)
+                const auto *m = table->try_get({material::id_type(*i), material::id_type(*j)});
+                if (!m) m = table->try_get({material::id_type(*j), material::id_type(*i)});
+                auto it = m_mixing.find(key);
+                if (!m) {
+                    if (it != m_mixing.end()) { del_a.push_back(*i); del_b.push_back(*j); m_mixing.erase(it); }
+                    continue;
+                }
+                if (m->spin_friction != 0 || m->roll_friction != 0 || m->stiffness < large_scalar || m->damping < large_scalar)
+                    throw std::runtime_error("stepper_b2d: material mixing entries with spin / roll friction, stiffness or damping are not supported");
+                const std::pair<float, float> v {float(m->friction), float(m->restitution)};
+                if (it != m_mixing.end() && it->second == v) continue;
+                m_mixing[key] = v;
+                set_a.push_back(*i); set_b.push_back(*j); set_f.push_back(v.first); set_r.push_back(v.second);
+            }
+        }
+        if ((!del_a.empty() || !set_a.empty()) && (!b2d_set_material_mixing || !b2d_remove_material_mixing))
+            throw std::runtime_error("stepper_b2d: the linked libb2d has no material mixing (b2d_set_material_mixing)");
+        if (!del_a.empty()) check(b2d_remove_material_mixing(m_world, uint32_t(del_a.size()), del_a.data(), del_b.data()), "b2d_remove_material_mixing");
+        if (!set_a.empty()) check(b2d_set_material_mixing(m_world, uint32_t(set_a.size()), set_a.data(), set_b.data(), set_f.data(), set_r.data()), "b2d_set_material_mixing");
     }
 
     // ---- device -> registry: what solver::update writes at the end of a step (island_solver.cpp:358-376,
@@ -351,10 +427,12 @@ public:
     // ---- stepper_sequential's public surface
     void step_simulation(double time) {                                // stepper_sequential.cpp:121-147 (one fixed step)
         auto &s = m_registry->ctx().get<settings>();
+        check_material_toggles();
         stage_new_bodies();
         stage_new_hinges();
         stage_exclusions();
         upload_dirty();
+        sync_material_table();
         if (s.pre_step_callback) (*s.pre_step_callback)(*m_registry);
         check(b2d_step(m_world, 1), "b2d_step");
         ++m_steps;
@@ -380,7 +458,8 @@ public:
     // A user who observes contacts calls mirror_contacts() when they want to look: afterwards the registry holds what
     // the CPU stepper would hold -- one contact_manifold + contact_manifold_state entity per touching (AABB-overlapping)
     // pair, and per contact point an entity with contact_point, contact_point_list, contact_point_geometry,
-    // contact_point_material and contact_point_impulse, linked newest first (collision_util.cpp:319-395).  A point keeps
+    // contact_point_material and contact_point_impulse -- the last two only where both bodies have a material (a sensor's
+    // points have neither, collision_util.cpp:358-384) -- linked newest first (collision_util.cpp:319-395).  A point keeps
     // its entity for as long as it persists on the device (matched through its lifetime counter and its place in the
     // list); new points get contact_started_tag after their components, like narrowphase::patch_new_contacts
     // (narrowphase.cpp:111-130); vanished points and manifolds are destroyed, so on_destroy<contact_point> fires.
@@ -410,12 +489,13 @@ public:
                 reg.emplace<contact_manifold_state>(me);
             }
             next.emplace(key, me);
-            sync_points(me, std::min<uint32_t>(num[i], 4u), &pt[72 * size_t(i)], &u2[8 * size_t(i)], elapsed, st);
+            const bool sensor = m_sensor[a] || m_sensor[b];
+            sync_points(me, std::min<uint32_t>(num[i], 4u), &pt[72 * size_t(i)], &u2[8 * size_t(i)], elapsed, sensor, st);
             ++st.manifolds;
         }
         for (auto &gone : m_manifold_of) {                                     // pairs that separated since the last look
             if (!reg.valid(gone.second)) continue;
-            sync_points(gone.second, 0, nullptr, nullptr, elapsed, st);
+            sync_points(gone.second, 0, nullptr, nullptr, elapsed, false, st);
             reg.destroy(gone.second);
         }
         m_manifold_of.swap(next);
@@ -424,7 +504,9 @@ public:
     }
 
 private:
-    void sync_points(entt::entity me, uint32_t np, const float *p18, const uint32_t *u2, uint32_t elapsed, mirror_stats &st) {
+    // sensor: a pair with a body without material, whose points have no contact_point_material and no contact_point_impulse
+    // (collision_util.cpp:358-384)
+    void sync_points(entt::entity me, uint32_t np, const float *p18, const uint32_t *u2, uint32_t elapsed, bool sensor, mirror_stats &st) {
         auto &reg = *m_registry;
         std::vector<entt::entity> old, now(np, entt::entity{entt::null}), fresh;
         for (auto e = reg.get<contact_manifold_state>(me).contact_entity; e != entt::null; e = reg.get<contact_point_list>(e).next) old.push_back(e);
@@ -443,8 +525,7 @@ private:
             }
             if (e == entt::null) {
                 e = reg.create();
-                reg.emplace<contact_point_material>(e);
-                reg.emplace<contact_point_impulse>(e);
+                if (!sensor) { reg.emplace<contact_point_material>(e); reg.emplace<contact_point_impulse>(e); }
                 reg.emplace<contact_point_geometry>(e);
                 reg.emplace<contact_point_list>(e);
                 reg.emplace<contact_point>(e);
@@ -456,10 +537,12 @@ private:
             auto &geom = reg.get<contact_point_geometry>(e);
             geom.local_normal = {p[9], p[10], p[11]}; geom.distance = p[12];
             geom.normal_attachment = static_cast<contact_normal_attachment>(u2[2 * s]);
-            auto &mat = reg.get<contact_point_material>(e);
-            mat.friction = p[13]; mat.restitution = p[14]; mat.spin_friction = 0; mat.roll_friction = 0;
-            auto &imp = reg.get<contact_point_impulse>(e);
-            imp.normal_impulse = p[15]; imp.friction_impulse = {p[16], p[17]};
+            if (!sensor) {
+                auto &mat = reg.get<contact_point_material>(e);
+                mat.friction = p[13]; mat.restitution = p[14]; mat.spin_friction = 0; mat.roll_friction = 0;
+                auto &imp = reg.get<contact_point_impulse>(e);
+                imp.normal_impulse = p[15]; imp.friction_impulse = {p[16], p[17]};
+            }
             now[s] = e;
             ++st.points;
         }

@@ -37,10 +37,15 @@ def plane_shape(normal, constant):
     return Shape(SHAPE_PLANE, (normal[0], normal[1], normal[2], constant))
 
 
+MATERIAL_UNASSIGNED = 0xFFFF           # material::UnassignedID
+MATERIAL_NONE = 0xFFFFFFFF             # B2D_MATERIAL_NONE: no material component, the body is a sensor
+
+
 @dataclass
 class Material:                        # include/edyn/comp/material.hpp (friction default 0.5, restitution 0)
     restitution: float = 0.0
     friction: float = 0.5
+    id: int = MATERIAL_UNASSIGNED      # material::id, the key of the mixing table (edyn.insert_material_mixing)
 
 
 @dataclass
@@ -54,7 +59,7 @@ class RigidBodyDef:                    # include/edyn/util/rigidbody.hpp rigidbo
     angvel: Sequence[float] = (0.0, 0.0, 0.0)
     gravity: Optional[Sequence[float]] = None      # None -> world default (settings.gravity)
     shape: Optional[Shape] = None
-    material: Optional[Material] = field(default_factory=Material)
+    material: Optional[Material] = field(default_factory=Material)     # None: a sensor (collides, is never pushed)
     collision_group: int = 0xFFFFFFFFFFFFFFFF
     collision_mask: int = 0xFFFFFFFFFFFFFFFF
 
@@ -122,7 +127,8 @@ def bodies_soa(defs: Sequence[RigidBodyDef], default_gravity=(0.0, -9.8, 0.0)) -
                angvel=np.zeros((n, 3), f32), inv_mass=np.zeros(n, f32), inv_inertia=np.zeros((n, 9), f32),
                gravity=np.zeros((n, 3), f32), kind=np.zeros(n, np.uint32), shape_kind=np.full(n, SHAPE_NONE, np.uint32),
                shape_params=np.zeros((n, 4), f32), friction=np.zeros(n, f32), restitution=np.zeros(n, f32),
-               group=np.full(n, 0xFFFFFFFFFFFFFFFF, np.uint64), mask=np.full(n, 0xFFFFFFFFFFFFFFFF, np.uint64))
+               group=np.full(n, 0xFFFFFFFFFFFFFFFF, np.uint64), mask=np.full(n, 0xFFFFFFFFFFFFFFFF, np.uint64),
+               material=np.full(n, MATERIAL_UNASSIGNED, np.uint32))
     cache = {}
     for i, d in enumerate(defs):
         out["pos"][i] = d.position
@@ -149,6 +155,9 @@ def bodies_soa(defs: Sequence[RigidBodyDef], default_gravity=(0.0, -9.8, 0.0)) -
         if d.material is not None:
             out["friction"][i] = d.material.friction
             out["restitution"][i] = d.material.restitution
+            out["material"][i] = d.material.id
+        else:
+            out["material"][i] = MATERIAL_NONE
         out["group"][i] = d.collision_group
         out["mask"][i] = d.collision_mask
     return out

@@ -6,6 +6,7 @@ Mirrors the reference's lifecycle surface for the sequential stepper
     make_rigidbody(world, def)        edyn::make_rigidbody(registry, def)
     make_hinge(world, a, b, ...)      edyn::make_constraint<hinge_constraint>(...) + set_axes
     exclude_collision(world, a, b)    edyn::exclude_collision
+    insert_material_mixing(world, id0, id1, material)   edyn::insert_material_mixing
     step_simulation(world)            edyn::step_simulation(registry, t)   (one fixed step)
     update(world, dt_elapsed)         edyn::update(registry, time)         (accumulator, <= max_steps)
     set_solver_velocity_iterations... edyn::set_solver_velocity_iterations
@@ -17,7 +18,7 @@ import numpy as np
 
 from . import _lib
 from ._lib import B2DError, Bodies, BodyPatch, Config, Stats
-from .rigidbody import RigidBodyDef, bodies_soa
+from .rigidbody import MATERIAL_UNASSIGNED, Material, RigidBodyDef, bodies_soa
 
 f32, u32 = np.float32, np.uint32
 
@@ -92,9 +93,10 @@ class World:
                     restitution=_c(soa["restitution"], f32, (n,)))
         grp = _c(soa["group"], np.uint64, (n,)) if soa.get("group") is not None else None
         msk = _c(soa["mask"], np.uint64, (n,)) if soa.get("mask") is not None else None
+        mat = _c(soa["material"], u32, (n,)) if soa.get("material") is not None else None     # absent: all unassigned
         b = Bodies(n, *[_p(keep[k]) for k in ("pos", "orn", "linvel", "angvel", "inv_mass", "inv_inertia", "gravity",
                                                "kind", "shape_kind", "shape_params", "friction", "restitution")],
-                   _p(grp), _p(msk))
+                   _p(grp), _p(msk), _p(mat))
         first = C.c_uint32(0)
         self._check(self.l.b2d_add_bodies(self.h, C.byref(b), C.byref(first)))
         self.num_bodies += n
@@ -102,6 +104,7 @@ class World:
         keep["group"] = grp if grp is not None else np.full(n, ~np.uint64(0), np.uint64)
         keep["mask"] = msk if msk is not None else np.full(n, ~np.uint64(0), np.uint64)
         keep["has_filter"] = np.full(n, grp is not None and msk is not None, bool)
+        keep["material"] = mat if mat is not None else np.full(n, MATERIAL_UNASSIGNED, u32)
         self._defs.append(keep)
         return first.value
 
@@ -194,20 +197,33 @@ class World:
 
     def upload_bodies(self, ids, **comp):
         """registry.patch on a subset of bodies (b2d_upload_bodies): comp = pos / orn / linvel / angvel / inv_mass /
-        inv_inertia / gravity / friction / restitution / kind, each packed per listed body; the rest stays untouched."""
+        inv_inertia / gravity / friction / restitution / kind / material, each packed per listed body; the rest stays
+        untouched.  material: ids (MATERIAL_NONE for a sensor; a body cannot change between sensor and non-sensor)."""
         ids = _c(ids, u32)
         n = len(ids)
         shapes = dict(pos=(n, 3), orn=(n, 4), linvel=(n, 3), angvel=(n, 3), inv_mass=(n,), inv_inertia=(n, 9),
                       gravity=(n, 3), friction=(n,), restitution=(n,))
-        unknown = set(comp) - set(shapes) - {"kind"}
+        unknown = set(comp) - set(shapes) - {"kind", "material"}
         if unknown:
             raise B2DError(f"upload_bodies: unknown components {sorted(unknown)}")
         keep = {k: _c(v, f32, shapes[k]) for k, v in comp.items() if k in shapes}
-        if "kind" in comp:
-            keep["kind"] = _c(comp["kind"], u32, (n,))
+        for k in ("kind", "material"):
+            if k in comp:
+                keep[k] = _c(comp[k], u32, (n,))
         patch = BodyPatch(*[_p(keep.get(k)) for k in ("pos", "orn", "linvel", "angvel", "inv_mass", "inv_inertia", "gravity",
-                                                      "friction", "restitution", "kind")])
+                                                      "friction", "restitution", "kind", "material")])
         self._check(self.l.b2d_upload_bodies(self.h, C.c_uint32(n), _p(ids), C.byref(patch)))
+
+    def set_material_mixing(self, id0, id1, friction, restitution):
+        """material_mix_table::insert for the unordered id pairs (id0[i], id1[i]); applies to contact points created later."""
+        a, b = _c(id0, u32).reshape(-1), _c(id1, u32).reshape(-1)
+        f, r = _c(friction, f32, (len(a),)), _c(restitution, f32, (len(a),))
+        self._check(self.l.b2d_set_material_mixing(self.h, C.c_uint32(len(a)), _p(a), _p(b), _p(f), _p(r)))
+
+    def remove_material_mixing(self, id0, id1):
+        """material_mix_table::remove for the unordered id pairs (id0[i], id1[i]); absent pairs are ignored."""
+        a, b = _c(id0, u32).reshape(-1), _c(id1, u32).reshape(-1)
+        self._check(self.l.b2d_remove_material_mixing(self.h, C.c_uint32(len(a)), _p(a), _p(b)))
 
     def download_state(self, aabb=True, inv_IW=False, out=None):
         n = self.num_bodies
@@ -394,6 +410,12 @@ def make_hinge(world: World, body_a, body_b, pivot_a, pivot_b, axis_a, axis_b):
 def exclude_collision(world: World, a, b):
     """edyn::exclude_collision (src/edyn/util/exclude_collision.cpp)."""
     world.add_exclusions([a], [b])
+
+
+def insert_material_mixing(world: World, id0: int, id1: int, material: Material):
+    """edyn::insert_material_mixing (src/edyn/util/insert_material_mixing.cpp:9-22): friction and restitution of the contact
+    points created from now on between bodies of material ids id0 and id1 (either order)."""
+    world.set_material_mixing([id0], [id1], [material.friction], [material.restitution])
 
 
 def remove_collision_exclusion(world: World, a, b):

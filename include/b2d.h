@@ -44,6 +44,10 @@ extern "C" {
 #define B2D_ATTACH_A    1u
 #define B2D_ATTACH_B    2u
 
+/* b2d_bodies.material / b2d_body_patch.material values besides a material::id 0..0xFFFE (include/edyn/comp/material.hpp). */
+#define B2D_MATERIAL_UNASSIGNED 0xFFFFu      /* material::UnassignedID: the body has a material without an id */
+#define B2D_MATERIAL_NONE 0xFFFFFFFFu        /* no material component: the body is a sensor */
+
 /* b2d_run_phases() mask: the four calls of stepper_sequential.cpp:82-91. */
 #define B2D_PHASE_BROAD   1u
 #define B2D_PHASE_NARROW  2u
@@ -83,7 +87,12 @@ typedef struct b2d_config {
 
 /* make_rigidbody() output for n bodies (src/edyn/util/rigidbody.cpp:47-185), SoA.
  * inv_inertia = inertia_inv component, row-major 3x3 in body space (ignored unless dynamic).
- * gravity = gravity component (zero if absent).  group/mask may be NULL (= no collision_filter). */
+ * gravity = gravity component (zero if absent).  group/mask may be NULL (= no collision_filter).
+ * material: n values or NULL (= every body B2D_MATERIAL_UNASSIGNED).  A material id, B2D_MATERIAL_UNASSIGNED, or
+ *   B2D_MATERIAL_NONE: an empty rigidbody_def::material, a sensor (util/collision_util.cpp:358-384,
+ *   util/constraint_util.cpp:82-85).  A sensor's pairs get manifolds and contact points like any other pair, join and keep
+ *   awake islands like them, but get no contact constraint: nothing pushes or bounces on a sensor, and its friction and
+ *   restitution are not read.  Other values: B2D_ERR_ARGUMENT. */
 typedef struct b2d_bodies {
     uint32_t count;
     const float *pos;          /* 3n  position */
@@ -100,6 +109,7 @@ typedef struct b2d_bodies {
     const float *restitution;  /* n   material.restitution */
     const uint64_t *group;     /* n or NULL  collision_filter.group */
     const uint64_t *mask;      /* n or NULL  collision_filter.mask */
+    const uint32_t *material;  /* n or NULL  material.id, B2D_MATERIAL_UNASSIGNED or B2D_MATERIAL_NONE (sensor) */
 } b2d_bodies;
 
 /* profile_counters + profile_timers analogue (include/edyn/context/profile.hpp:8-27). */
@@ -152,8 +162,24 @@ typedef struct b2d_body_patch {
     const float *gravity;                       /* 3n */
     const float *friction, *restitution;        /* n  n  */
     const uint32_t *kind;                       /* n  */
+    const uint32_t *material;                   /* n  material.id; a change between B2D_MATERIAL_NONE and a material
+                                                      (sensor <-> non-sensor) is B2D_ERR_UNSUPPORTED */
 } b2d_body_patch;
 int b2d_upload_bodies(b2d_world *w, uint32_t n, const uint32_t *body_ids, const b2d_body_patch *patch);
+
+/* insert_material_mixing / material_mix_table::remove (util/insert_material_mixing.cpp:9-22, dynamics/material_mixing.hpp:36-80)
+ * for n unordered id pairs (id0[i], id1[i]).  An insert overwrites an existing entry; removing an absent pair is ignored.
+ * Ids >= 0xFFFF are B2D_ERR_ARGUMENT (the reference asserts on them).  When a contact point is created and both bodies
+ * have materials, the entry of their two ids replaces the mixed friction sqrt(fA fB) and restitution min(rA, rB)
+ * (collision_util.cpp:282-317); existing points keep theirs, as in the reference.  The table is per world: a host
+ * framework that spreads a scene over several worlds (island hand-over) sets the same table on every one.
+ * Known difference: whether the restitution solver (B2D_FLAG_RESTITUTION_SOLVER) treats a manifold as one with
+ * restitution is evaluated every step from the table and the bodies' materials; the reference fixes it when the manifold
+ * is created (constraint_util.cpp:90-101).  A table edit or a restitution patch reaches existing manifolds at once here,
+ * only new ones in the reference. */
+int b2d_set_material_mixing(b2d_world *w, uint32_t n, const uint32_t *id0, const uint32_t *id1, const float *friction,
+                            const float *restitution);
+int b2d_remove_material_mixing(b2d_world *w, uint32_t n, const uint32_t *id0, const uint32_t *id1);
 
 /* n fixed steps: broadphase -> narrowphase -> islands -> solve/integrate (step_simulation semantics). */
 int b2d_step(b2d_world *w, uint32_t num_steps);
@@ -173,7 +199,9 @@ int b2d_download_state(b2d_world *w, float *pos, float *orn, float *linvel, floa
  * distance friction restitution normal_impulse friction_impulse[2]; pt_u2 = {normal_attachment, lifetime}.
  * A point stores its attachment and lifetime in one 32-bit word: b2d_upload_contacts returns B2D_ERR_ARGUMENT for a
  * normal_attachment > 2 or a lifetime >= 2^30 in any of the first num slots.  The step counts a lifetime modulo 2^30
- * (about 207 days at 60 Hz) where the reference's uint32 would go on; nothing in the step reads it. */
+ * (about 207 days at 60 Hz) where the reference's uint32 would go on; nothing in the step reads it.
+ * A sensor's points (B2D_MATERIAL_NONE on either body) have no contact_point_material and no contact_point_impulse: their
+ * friction, restitution and impulses are reported as 0. */
 int b2d_num_manifolds(b2d_world *w, uint32_t *n);
 int b2d_download_pairs(b2d_world *w, uint32_t capacity, uint32_t *pairs, uint32_t *n);
 int b2d_download_contacts(b2d_world *w, uint32_t capacity, uint32_t *pairs, uint32_t *num,
