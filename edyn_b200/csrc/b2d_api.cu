@@ -193,6 +193,8 @@ b2d_world *b2d_create(const b2d_config *cfg) {
     d.isl_nm = d.isl_nb + NB; d.isl_nh = d.isl_nb + 2 * (size_t)NB;
     ok = ok && dalloc(w, d.tile_nb, 5 * (size_t)d.max_tiles) && dalloc(w, d.tile_body, (size_t)d.max_tiles * TILE_CAP);
     d.tile_c0 = d.tile_nb + d.max_tiles; d.tile_c1 = d.tile_c0 + d.max_tiles; d.tile_h0 = d.tile_c1 + d.max_tiles; d.tile_h1 = d.tile_h0 + d.max_tiles;
+    ok = ok && dalloc(w, d.tile_hdr, d.max_tiles) && dalloc(w, d.tplan_h, (size_t)d.max_tiles * TILE_CAP) && dalloc(w, d.tplan_c, (size_t)d.max_tiles * TILE_CAP);
+    ok = ok && dalloc(w, d.tplan_w, (size_t)d.max_tiles * TILE_CAP);
     ok = ok && dalloc(w, d.isl_err, NB) && dalloc(w, d.isl_done, NB);
     ok = ok && dalloc(w, d.hdr, NM) && dalloc(w, d.R0, 4 * (size_t)NM) && dalloc(w, d.R1, 4 * (size_t)NM) && dalloc(w, d.R2, 4 * (size_t)NM);
     ok = ok && dalloc(w, d.R3, 4 * (size_t)NM) && dalloc(w, d.IMP, 4 * (size_t)NM);
@@ -737,6 +739,7 @@ static int enqueue_rebuild(b2d_world *w, int recolor) {
     CK(cub::DeviceRadixSort::SortPairs(w->cub_tmp, t, d.hkey, d.hkey_s, d.hidx, d.hidx_s, (int)d.NH, 0, COLOR_KEY_BITS, s)); w->launches += 3;
     LAUNCH(k_color_offsets, d.NM, 256, d);
     LAUNCH(k_color_fixup, 1, 32, d);
+    if (d.max_tiles) LAUNCH(k_tile_plan, (uint64_t)d.max_tiles * TILE_CAP, TILE_CAP, d);
     return B2D_OK;
 }
 static int enqueue_prepare(b2d_world *w) {

@@ -1292,7 +1292,8 @@ B2D_D void hinge_rows(const Dev &d, uint32_t h, const SBody &A, const SBody &B, 
 
 // Row header of a sorted constraint (Dev::hdr / hhdr): the tags of bodies a and b, the point count or hinge id, and the
 // bodies' slots in an island tile.  A body tag is the body id, with the top bit set for a body the solver does not move.
-B2D_D uint32_t body_tag(uint32_t id, const SBody &b) { return id | (b.proc ? 0u : 0x80000000u); }
+B2D_D uint32_t body_tag(uint32_t id, bool proc) { return id | (proc ? 0u : 0x80000000u); }
+B2D_D uint32_t body_tag(uint32_t id, const SBody &b) { return body_tag(id, b.proc); }
 B2D_D uint32_t tag_id(uint32_t tag) { return tag & 0x7FFFFFFFu; }
 B2D_D bool tag_proc(uint32_t tag) { return !(tag >> 31); }
 B2D_D uint32_t slot_pair(uint32_t sa, uint32_t sb) { return sa | (sb << 16); }
@@ -1871,7 +1872,8 @@ B2D_D void tile_error_max(uint32_t *s_err, uint32_t islot, float err) { if (err 
 // velocity iterations run, the bodies are integrated
 // where they sit (shared memory), the impulses go straight to the warm-start cache, the position iterations run on
 // the same records, and positions / orientations / velocities are written once.  One CTA per tile; thread t owns joint t
-// and manifold t of the tile for all iterations, and colours are separated by __syncthreads instead of tickets.  The row,
+// and manifold t of the tile for all iterations (as the lane plan of k_tile_plan lists them), and colours are separated
+// by __syncthreads instead of tickets.  The row,
 // solve, integration and position functions are those of the separate kernels, called in the same order
 // (k_prepare_contacts, k_prepare_hinges, k_integrate, k_store_impulses, k_finalize skip what this kernel has done).  Without
 // position iterations the position loop does not run and the integrated pose is written back.  Either way the AABBs and
@@ -1911,12 +1913,11 @@ B2D_D FJac tile_fjac_load(const float4 *fj, uint32_t t, int p) {
     f.U1 = mk3(e.x, e.y, e.z); f.U3 = mk3(e.w, g.x, g.y);
     return f;
 }
-// solver_body (+ position, orientation, record slot) of body `id` of a tiled constraint during the row preparation: a
-// dynamic body from the records staged by slot, a static / kinematic one from global memory
-B2D_D void tile_solver_body(const Dev &d, const float4 *sb, uint32_t id, SBody &s, v3 &pos, q4 &orn, uint32_t &slot) {
-    const uint32_t f = d.flags[id];
-    if (!is_dynamic(f)) { s = solver_body(d, id, f); pos = mk3(d.pos[id]); orn = mkq(d.orn[id]); slot = SLOT_NONE; return; }
-    slot = d.bslot[id];
+// solver_body (+ position, orientation) of the body of a tiled constraint with tag `tag` and record slot `slot` (from the
+// lane plan) during the row preparation: a dynamic body from the records staged by slot, a static / kinematic one from
+// global memory
+B2D_D void tile_solver_body(const Dev &d, const float4 *sb, uint32_t tag, uint32_t slot, SBody &s, v3 &pos, q4 &orn) {
+    if (!tag_proc(tag)) { const uint32_t id = tag_id(tag); s = solver_body(d, id, d.flags[id]); pos = mk3(d.pos[id]); orn = mkq(d.orn[id]); return; }
     const float4 r0 = sb[2 * TILE_CAP + slot];
     s.proc = true; s.inv_m = r0.w;
     s.inv_I.r0 = mk3(r0); s.inv_I.r1 = mk3(sb[3 * TILE_CAP + slot]); s.inv_I.r2 = mk3(sb[4 * TILE_CAP + slot]);
@@ -1948,6 +1949,40 @@ B2D_D void tq_store(float4 *sb, uint32_t slot, const PBody &b) {
     sb[slot] = f4(b.pos, b.inv_m); sb[TILE_CAP + slot] = f4(b.orn);
     sb[2 * TILE_CAP + slot] = f4(b.inv_IW.r0, 0); sb[3 * TILE_CAP + slot] = f4(b.inv_IW.r1, 0); sb[4 * TILE_CAP + slot] = f4(b.inv_IW.r2, 0);
 }
+// Lane plan of the island tiles, the last kernel of the island rebuild: for lane t of every tile, what the tile kernels
+// would otherwise find by chasing indices at every step (cidx_s / hidx_s, then mpair / hpair, then flags and bslot of
+// both bodies, then parent and bslot of the island root).  Every input is an output of the rebuild or changes only
+// with graph_changed set, so the plan is valid exactly as long as the rest of the rebuild's results (DESIGN §2).
+B2D_D uint4 tile_lane(const Dev &d, uint2 pr, uint32_t id, uint32_t col, uint32_t &w) {
+    const bool pa = is_dynamic(d.flags[pr.x]), pb = is_dynamic(d.flags[pr.y]);
+    w = col | d.bslot[island_of(d, pr.x, pr.y)] << 16;
+    return make_uint4(body_tag(pr.x, pa), body_tag(pr.y, pb), id, slot_pair(pa ? d.bslot[pr.x] : SLOT_NONE, pb ? d.bslot[pr.y] : SLOT_NONE));
+}
+__global__ void __launch_bounds__(TILE_CAP) k_tile_plan(Dev d) {
+    __shared__ uint32_t s_ncol[2];
+    const uint32_t ntiles = d.cnt->ntiles, t = threadIdx.x;
+    for (uint32_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+        if (t == 0) s_ncol[0] = s_ncol[1] = 0;          // thread 0 read the previous tile's counts before this
+        __syncthreads();
+        const uint32_t c0 = d.tile_c0[tile], c1 = min(d.tile_c1[tile], c0 + TILE_CAP), h0 = d.tile_h0[tile], h1 = min(d.tile_h1[tile], h0 + TILE_CAP);
+        const size_t k = (size_t)tile * TILE_CAP + t;
+        uint2 w = make_uint2(0, 0);
+        if (h0 + t < h1) {
+            const uint32_t h = d.hidx_s[h0 + t], col = d.hkey_s[h0 + t] & 63u;
+            d.tplan_h[k] = tile_lane(d, d.hpair[h], h, col, w.x);
+            atomicMax(&s_ncol[0], col + 1u);
+        }
+        if (c0 + t < c1) {
+            const uint32_t m = d.cidx_s[c0 + t], col = d.ckey_s[c0 + t] & 63u;
+            d.tplan_c[k] = tile_lane(d, d.mpair[m], m, col, w.y);
+            atomicMax(&s_ncol[1], col + 1u);
+        }
+        d.tplan_w[k] = w;
+        __syncthreads();
+        if (t == 0) d.tile_hdr[tile] = make_uint4(min(d.tile_nb[tile], (uint32_t)TILE_CAP), h1 > h0 ? h1 - h0 : 0u, c1 > c0 ? c1 - c0 : 0u,
+                                                  s_ncol[0] | s_ncol[1] << 16);
+    }
+}
 template <int MAXP>
 B2D_D void island_tiles(const Dev &d, int vel_iters, int pos_iters) {
     constexpr bool TWO = MAXP == 2;
@@ -1956,49 +1991,53 @@ B2D_D void island_tiles(const Dev &d, int vel_iters, int pos_iters) {
     float4 *s_p2 = s_tile + 5 * TILE_CAP + threadIdx.x, *s_pt = s_tile + 8 * TILE_CAP + threadIdx.x;       // two-point only
     float4 *s_fj = s_tile + 17 * TILE_CAP;
     __shared__ uint32_t s_err[TILE_CAP], s_done[TILE_CAP], s_root[TILE_CAP];
-    __shared__ uint32_t s_ncol[2];
     const uint32_t tile0 = TWO ? 0u : d.cnt->ntiles2, ntiles = TWO ? d.cnt->ntiles2 : d.cnt->ntiles, t = threadIdx.x;
     const size_t NM = d.NM;
     for (uint32_t tile = tile0 + blockIdx.x; tile < ntiles; tile += gridDim.x) {
-        const uint32_t nb = min(d.tile_nb[tile], (uint32_t)TILE_CAP);
-        const uint32_t c0 = d.tile_c0[tile], c1 = min(d.tile_c1[tile], c0 + TILE_CAP), h0 = d.tile_h0[tile], h1 = min(d.tile_h1[tile], h0 + TILE_CAP);
-        if (t < 2) s_ncol[t] = 0;
-        uint32_t mybody = 0;
+        // The tile header, the slot's body and the lane plan (k_tile_plan) come first, then every gather by the ids they
+        // hold.  Lanes past a count read plan rows they do not use.
+        const uint32_t lane = tile * TILE_CAP + t;
+        const uint4 th = d.tile_hdr[tile];
+        const uint32_t mybody = d.tile_body[lane];
+        uint4 hh = d.tplan_h[lane], ch = d.tplan_c[lane];      // tags, hinge id | manifold slot, body slots
+        const uint2 pw = d.tplan_w[lane];
+        const uint32_t nb = th.x, nhc = th.w & 0xFFFFu, ncc = th.w >> 16;
+        const bool hasH = t < th.y, hasC = t < th.z;
+        const uint32_t hcol = hasH ? pw.x & 0xFFFFu : 0xFFu, ccol = hasC ? pw.y & 0xFFFFu : 0xFFu;
+        if (!hasH) hh = make_uint4(0, 0, 0, 0);
+        if (!hasC) ch = make_uint4(0, 0, 0, 0);
         if (t < nb) {       // body state for the row preparation, by slot; the velocities sit where dv, dw go until it ends
-            mybody = d.tile_body[(size_t)tile * TILE_CAP + t];
             s_body[t] = d.linvel[mybody]; s_body[TILE_CAP + t] = d.angvel[mybody];
             s_body[2 * TILE_CAP + t] = d.invIW[3 * mybody]; s_body[3 * TILE_CAP + t] = d.invIW[3 * mybody + 1]; s_body[4 * TILE_CAP + t] = d.invIW[3 * mybody + 2];
             s_body[5 * TILE_CAP + t] = d.pos[mybody]; s_body[6 * TILE_CAP + t] = d.orn[mybody];
             s_err[t] = 0; s_done[t] = 0; s_root[t] = d.parent[mybody] == mybody ? 1u : 0u;
         }
+        const uint32_t npts = hasC ? d.mstate[ch.z] & MS_NPTS_MASK : 0u;
+        // the lines the row preparation reads by hinge id and manifold slot are requested now, so that they arrive while the
+        // body state is staged
+        if (hasH) { const uint32_t h = hh.z; prefetch_L2(&d.hpivA[h]); prefetch_L2(&d.hpivB[h]); prefetch_L2(&d.hfA1[h]); prefetch_L2(&d.hfA2[h]); prefetch_L2(&d.himp[5 * (size_t)h]); prefetch_L2(&d.himp[5 * (size_t)h + 4]); }
+        if (hasC) {
+            const uint32_t m = ch.z;
+            prefetch_L2(&d.pA[m]); prefetch_L2(&d.pB[m]); prefetch_L2(&d.pN[m]); prefetch_L2(&d.pI[m]);
+            if (npts > 1) { prefetch_L2(&d.pA[NM + m]); prefetch_L2(&d.pB[NM + m]); prefetch_L2(&d.pN[NM + m]); prefetch_L2(&d.pI[NM + m]); }
+        }
         __syncthreads();
-        const bool hasH = h0 + t < h1, hasC = c0 + t < c1;
-        const uint32_t hi = h0 + t, ci = c0 + t;
-        uint4 hh = make_uint4(0, 0, 0, 0), ch = make_uint4(0, 0, 0, 0);
-        uint32_t hcol = 0xFFu, ccol = 0xFFu;
         float4 a0, a1, a2, a3, aim, b0, b1, b2, b3, bim;      // rows of contact points 1 and 2
         a0 = a1 = a2 = a3 = aim = b0 = b1 = b2 = b3 = bim = make_float4(0, 0, 0, 0);
         // ---- row preparation (k_prepare_hinges / k_prepare_contacts of the tiled range): rows go straight to where the
-        // solve keeps them; hh / ch are the row headers those kernels write (tags, hinge id | point count, body slots)
+        // solve keeps them; hh / ch become the row headers those kernels write (tags, hinge id | point count, body slots)
         if (hasH) {
-            const uint32_t h = d.hidx_s[hi];
-            const uint2 pr = d.hpair[h];
-            SBody A, B; v3 posA, posB; q4 ornA, ornB; uint32_t sa, sb;
-            tile_solver_body(d, s_body, pr.x, A, posA, ornA, sa); tile_solver_body(d, s_body, pr.y, B, posB, ornB, sb);
-            hinge_rows(d, h, A, B, posA, ornA, posB, ornB, s_hr + t, TILE_CAP);
-            hh = make_uint4(body_tag(pr.x, A), body_tag(pr.y, B), h, slot_pair(sa, sb));
-            hcol = d.hkey_s[hi] & 63u;
-            atomicMax(&s_ncol[0], hcol + 1u);
+            SBody A, B; v3 posA, posB; q4 ornA, ornB;
+            tile_solver_body(d, s_body, hh.x, slot_a(hh.w), A, posA, ornA); tile_solver_body(d, s_body, hh.y, slot_b(hh.w), B, posB, ornB);
+            hinge_rows(d, hh.z, A, B, posA, ornA, posB, ornB, s_hr + t, TILE_CAP);
         }
         if (hasC) {
-            const uint32_t m = d.cidx_s[ci];
-            const uint2 pr = d.mpair[m];
-            const uint32_t npts = d.mstate[m] & MS_NPTS_MASK;
-            SBody A, B; v3 posA, posB; q4 ornA, ornB; uint32_t sa, sb;
-            tile_solver_body(d, s_body, pr.x, A, posA, ornA, sa); tile_solver_body(d, s_body, pr.y, B, posB, ornB, sb);
+            const uint32_t m = ch.z;
+            SBody A, B; v3 posA, posB; q4 ornA, ornB;
+            tile_solver_body(d, s_body, ch.x, slot_a(ch.w), A, posA, ornA); tile_solver_body(d, s_body, ch.y, slot_b(ch.w), B, posB, ornB);
             // a two-point tile holds no manifold with more points: one that gains a third point sets graph_changed
             // (np_merge) and the rebuild moves its island to a generic tile before the next solve
-            ch = make_uint4(body_tag(pr.x, A), body_tag(pr.y, B), TWO ? min(npts, 2u) : npts, slot_pair(sa, sb));
+            ch.z = TWO ? min(npts, 2u) : npts;
             if (TWO) {      // rA, rB give way to the normal row's J1, J3; the friction Jacobians go to s_fj
                 v3 J1, J3; FJac fj;
                 contact_point_rows(d, m, A, B, posA, ornA, posB, ornB, a0, a1, a2, a3, aim, J1, J3, fj);
@@ -2015,14 +2054,11 @@ B2D_D void island_tiles(const Dev &d, int vel_iters, int pos_iters) {
                 float4 *r = s_row + (s - 2) * 5 * TILE_CAP + t;
                 contact_point_rows(d, s * NM + m, A, B, posA, ornA, posB, ornB, r[0], r[TILE_CAP], r[2 * TILE_CAP], r[3 * TILE_CAP], r[4 * TILE_CAP]);
             }
-            ccol = d.ckey_s[ci] & 63u;
-            atomicMax(&s_ncol[1], ccol + 1u);
         }
         __syncthreads();
         if (t < nb) { s_body[t] = make_float4(0, 0, 0, 0); s_body[TILE_CAP + t] = make_float4(0, 0, 0, 0); }
         if (TWO && ch.z > 1) { s_p2[0] = b0; s_p2[TILE_CAP] = b1; s_p2[2 * TILE_CAP] = b2; s_p2[3 * TILE_CAP] = b3; s_p2[4 * TILE_CAP] = bim; }
         __syncthreads();
-        const uint32_t nhc = s_ncol[0], ncc = s_ncol[1];
         // the normal rows and the friction rows of this thread's manifold
         auto normals = [&](VBody &A, VBody &B, bool warm) {
             if (TWO) {
@@ -2101,9 +2137,10 @@ B2D_D void island_tiles(const Dev &d, int vel_iters, int pos_iters) {
             }
         }
         // ---- assign_applied_impulses (k_store_impulses): rows -> warm-start cache of the constraints
-        uint32_t m = 0;
+        uint32_t m = 0, hisl = 0, cisl = 0;          // the manifold slot and the island root slots from the plan, read again
+        if (hasH) hisl = d.tplan_w[lane].x >> 16;
         if (hasC) {
-            m = d.cidx_s[ci];
+            m = d.tplan_c[lane].z; cisl = d.tplan_w[lane].y >> 16;
             d.pI[m] = aim; if (ch.z > 1) d.pI[NM + m] = TWO ? s_p2[4 * TILE_CAP] : bim;
             if (!TWO) for (uint32_t s = 2; s < ch.z; ++s) d.pI[s * NM + m] = s_row[((s - 2) * 5 + 4) * TILE_CAP + t];
         }
@@ -2113,22 +2150,17 @@ B2D_D void island_tiles(const Dev &d, int vel_iters, int pos_iters) {
             imp[0] = r5.z; imp[1] = r5.w; imp[2] = r6.x; imp[3] = r6.y; imp[4] = r6.z;
         }
         // ---- what the position iterations need from global memory is requested before the integration below
-        uint32_t hisl = 0, cisl = 0;
         v3 fA0 = mk3(0, 0, 0), fB0 = fA0, pvA = fA0, pvB = fA0;
         float4 a40, b40, n40, l40, a41, b41, n41, l41;         // contact points 1 and 2
         a40 = b40 = n40 = l40 = a41 = b41 = n41 = l41 = make_float4(0, 0, 0, 0);
         float4 spos = make_float4(0, 0, 0, 0), sorn = make_float4(0, 0, 0, 1);      // this thread's non-procedural partner (contact, else joint)
         if (hasH) {
-            hisl = d.bslot[island_of(d, tag_id(hh.x), tag_id(hh.y))];
             const uint32_t h = hh.z;
             fA0 = mk3(d.hfA0[h]); fB0 = mk3(d.hfB0[h]); pvA = mk3(d.hpivA[h]); pvB = mk3(d.hpivB[h]);
         }
-        if (hasC) {
-            cisl = d.bslot[island_of(d, tag_id(ch.x), tag_id(ch.y))];
-            if (!TWO) {
-                a40 = d.pA[m]; b40 = d.pB[m]; n40 = d.pN[m]; l40 = d.pL[m];
-                if (ch.z > 1) { a41 = d.pA[NM + m]; b41 = d.pB[NM + m]; n41 = d.pN[NM + m]; l41 = d.pL[NM + m]; }
-            }
+        if (hasC && !TWO) {
+            a40 = d.pA[m]; b40 = d.pB[m]; n40 = d.pN[m]; l40 = d.pL[m];
+            if (ch.z > 1) { a41 = d.pA[NM + m]; b41 = d.pB[NM + m]; n41 = d.pN[NM + m]; l41 = d.pL[NM + m]; }
         }
         float4 hpos = spos, horn = sorn;                        // a joint to a static / kinematic body
         if (hasC && ((ch.x | ch.y) >> 31)) { const uint32_t sbody = tag_id(tag_proc(ch.x) ? ch.y : ch.x); spos = d.pos[sbody]; sorn = d.orn[sbody]; }
@@ -2197,9 +2229,9 @@ B2D_D void island_tiles(const Dev &d, int vel_iters, int pos_iters) {
             }
         }
         // the final pose, then update_aabbs + update_inertias of it (k_finalize and k_integrate skip tiled bodies), with
-        // inv_I from records 5-7; the body id is read again from the tile list rather than held across the iterations
+        // inv_I from records 5-7
         if (t < nb) {
-            const uint32_t i = d.tile_body[(size_t)tile * TILE_CAP + t];
+            const uint32_t i = mybody;
             const float4 p = s_body[t], o = s_body[TILE_CAP + t];
             const float inv_m = d.pos[i].w;
             d.pos[i] = make_float4(p.x, p.y, p.z, inv_m); d.orn[i] = o;

@@ -200,6 +200,14 @@ struct Dev {
     // hash of the unordered id pair (lo << 16 | hi) -> index into mix_mat (friction, restitution); mix_size slots
     uint32_t *matid;
     unsigned long long *mix_key; uint32_t *mix_idx; float2 *mix_mat; uint32_t mix_size;
+
+    // ---- island-tile lane plan (k_tile_plan, part of the island rebuild).  Per tile: bodies, hinge lanes, contact
+    // lanes, hinge colours | contact colours << 16.  Per tile lane (tile * TILE_CAP + t): the row header of hinge / manifold
+    // t of the tile (tags, hinge id / manifold slot, record slots), and for each of the two its colour | the record slot
+    // of its island's root << 16.
+    uint4 *tile_hdr;
+    uint4 *tplan_h, *tplan_c;
+    uint2 *tplan_w;
 };
 
 } // namespace b2d
