@@ -1,6 +1,7 @@
 """TEST INFRASTRUCTURE.  The command-line driver of the CPU emulation (tests/emu): the library's CUDA kernels, executed by
 the emulation, in lock step with the oracle through the normal Python adapter and C ABI -- the comparison of
-tests/parity.py, which the -m gpu tests make on the GPU (here the state is identical: glibc's sinf / cosf on both sides).
+tests/parity.py, which the -m gpu tests make on the GPU (here everything is bit-identical, the trig set's poses and
+contact normals included: glibc's sinf / cosf on both sides).
 
     python tests/emu/lockstep.py fixed|narrow|wide|large|beyond FIRST LAST [--tiles 0|1] [--steps N] [--restitution] [--mutate]
                                  [--bp-warp-max N]     -> one JSON line
@@ -103,6 +104,7 @@ def main():
     restitution = "--restitution" in sys.argv
     from tests.emu import build
     os.environ["B2D_LIB"] = build.build()
+    os.environ["B2D_EMU"] = "1"            # tests/parity.py: nothing is exempt from bit equality
     mode = "dataflow" if tiles == "0" else "plain"
     import edyn_b200 as E
     from oracle import oracle as O

@@ -43,17 +43,23 @@ def test_emulation_primitives(tmp_path):
     assert out.returncode == 0 and "emu selftest ok" in out.stdout, out.stdout + out.stderr
 
 
+def _bit_exact(res, steps):
+    """Under the emulation both sides call glibc's sinf / cosf: every step bit-identical, the trig set included."""
+    assert res["ok"] and res["worst"] == 0.0 and res["exact"] == steps, res
+    assert res["bitwise"] + res["trig"] > 0, res
+
+
 def test_emulated_kernels_on_the_benchmark_scene_families(O):
     """Validates the emulation itself: these five are green on a real GPU (tests/test_gpu_parity.py)."""
     for res in _run("fixed", 0, 5, steps=60):
-        assert res["ok"] and res["worst"] <= 1e-5, res
+        _bit_exact(res, 60)
     assert sum(r["points"] for r in _run("fixed", 1, 2, steps=60)) > 50
 
 
 @pytest.mark.parametrize("kind,first,last,tiles", [("narrow", 0, 2, "1"), ("wide", 0, 4, "1"), ("wide", 4, 6, "0"), ("narrow", 2, 3, "0")])
 def test_emulated_kernels_on_random_scenes(O, kind, first, last, tiles):
     for res in _run(kind, first, last, tiles=tiles):
-        assert res["ok"] and res["worst"] <= 1e-5, res
+        _bit_exact(res, 80)
 
 
 def test_emulated_restitution_solver(O):
@@ -62,13 +68,14 @@ def test_emulated_restitution_solver(O):
     real stepper (tests/test_ref_stepper.py).  The device fixes the orders the reference inherits from EnTT (neighbours in
     ascending body id, ties of the fastest manifold to the smaller pair key); the oracle's defaults are those conventions."""
     for res in _run("fixed", 3, 4, restitution=True) + _run("narrow", 0, 2, restitution=True) + _run("wide", 0, 3, restitution=True):
-        assert res["ok"] and res["worst"] <= 1e-5, res
+        _bit_exact(res, 80)
 
 
 def test_emulated_kernels_under_user_interference(O):
     """b2d_remove_bodies, b2d_add_bodies, b2d_remove_exclusions and b2d_upload_bodies every 13th step of random scenes."""
     for res in _run("narrow", 0, 2, steps=100, mutate=True):
-        assert res["ok"] and res["events"] >= 6, res
+        _bit_exact(res, 100)
+        assert res["events"] >= 6, res
 
 
 def test_emulated_kernels_against_the_real_stepper_directly(O):
@@ -92,7 +99,7 @@ def test_emulated_large_dynamic_bodies(O, tiles, search):
     res = _run("large", 0, 11, tiles=tiles, steps=12, extra=extra)
     assert len(res) == 11
     for r in res:
-        assert r["ok"] and r["worst"] == 0.0 and r["exact"] == 12, r
+        _bit_exact(r, 12)
         assert r["large"] and r["large"] == r["want"], r
         if r["scene"].startswith("plank_degree_"):
             assert r["colors"] == int(r["scene"].rsplit("_", 1)[1]), r

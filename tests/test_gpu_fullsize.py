@@ -1,10 +1,11 @@
 """Parity AT THE BENCHMARKED SIZES (BASELINE.json configs 2-5): the settled device state -- bodies, persistent contact
 manifolds with their warm-start impulses, joint impulses -- is loaded into the CPU oracle (exactly what bench.py's
 cpu_baseline leg does), then both sides step in lock step (tests/parity.py) and every phase is compared: ordered
-broadphase pair list, contact sets (point counts, attachments, lifetimes bit-equal; the point floats <= 1e-5), island
-partition, the post-solve state <= 1e-5 with the oracle replaying the device's colour order (within a colour the
-constraints touch disjoint dynamic bodies, so the coloured parallel solve IS a serial sweep in that order), and the
-post-solve contacts and joint impulses before they are copied into the oracle again."""
+broadphase pair list, contact sets, island partition, the post-solve state with the oracle replaying the device's colour
+order (within a colour the constraints touch disjoint dynamic bodies, so the coloured parallel solve IS a serial sweep in
+that order), and the post-solve contacts and joint impulses before they are copied into the oracle again -- all bit for
+bit, apart from the poses (and contact normals and distances) of the trig set of tests/parity.py.  So the island tiles
+and the dataflow solver are held to bits on every settled body whose step did not take integrate()'s sinf branch."""
 import os
 
 import numpy as np
@@ -13,7 +14,6 @@ import pytest
 from tests import parity as P
 
 pytestmark = pytest.mark.gpu
-STEP_TOL = 1e-5
 LOCKSTEP = 3
 
 FULL = {
@@ -34,8 +34,13 @@ def test_full_size_lockstep_parity(gpu, E, O, name):
     w.step(settle)
     o = P.oracle_for(O, scene, threads=os.cpu_count() or 1)
     P.load(o, w)
+    res = None
     for s in range(LOCKSTEP):
-        P.phase_step(E, O, w, o, s, STEP_TOL, partition=True)
+        res = P.tally(res, P.phase_step(E, O, w, o, s, partition=True))
+    # chains_1048576 leaves every body outside the trig set of tests/parity.py (3 x 1 048 576 poses compared bit for bit
+    # on an H100); in the settled piles some body of every island still turns by more than 0.001 rad/s, so all their
+    # poses are in it and what they hold to bits is the velocities, contacts, impulses, AABBs and inertias
+    P.report(name, res)
     st = w.stats()
     assert st["error_flags"] == 0, st
     assert st["contact_points"] > scene["dynamic"] // 4

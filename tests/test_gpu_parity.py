@@ -1,8 +1,9 @@
 """GPU parity tests proper: the CUDA path, called through the C ABI, against (a) the committed golden vectors generated
 from the real reference functions, (b) the CPU oracle on identical seeded inputs, and (c) size-independent properties
-at BASELINE.json's full sizes.  Bar: bit-exact for pair lists, island partitions and contact sets (integer / index work);
-<= 1e-5 absolute per step for positions/velocities (the library is built with -fmad=false, so in practice most steps are
-bit-identical; the residual comes from sinf/cosf differing from glibc by an ulp)."""
+at BASELINE.json's full sizes.  Bar (tests/parity.py): bit-exact for pair lists, island partitions, contact sets,
+velocities, hinge impulses, AABBs and inverse world inertias, and for poses outside the trig set -- the bodies whose
+step may have taken integrate()'s sinf / cosf, which may differ from glibc's by an ulp or two (the library is built with
+-fmad=false and otherwise restated operation for operation)."""
 import os
 
 import numpy as np
@@ -13,7 +14,6 @@ from tests import parity as P
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 f32 = np.float32
-STEP_TOL = 1e-5
 
 
 # ----------------------------------------------------------------------------- golden vectors from the reference
@@ -126,13 +126,13 @@ def test_lockstep_phase_parity(gpu, E, O, name):
     scene = make(E)
     w = E.scenes.build_world(scene)
     o = P.oracle_for(O, scene)
-    exact_steps = 0
+    res = None
     for s in range(steps):
         # every step a fresh single-step comparison: the oracle continues from the device's bodies, contacts and joints
-        errs = P.phase_step(E, O, w, o, s, STEP_TOL)
-        exact_steps += all(v == 0.0 for v in errs.values())
+        res = P.tally(res, P.phase_step(E, O, w, o, s))
+    P.report(name, res)
     assert w.stats()["error_flags"] == 0
-    assert exact_steps >= steps // 2, f"only {exact_steps}/{steps} steps were bit-identical"
+    assert res["bitwise"] > 0, res
 
 
 def test_solver_only_parity_from_injected_contacts(gpu, E, O):
@@ -147,8 +147,10 @@ def test_solver_only_parity_from_injected_contacts(gpu, E, O):
     w.upload_state(st["pos"], st["orn"], st["linvel"], st["angvel"])
     w.upload_contacts(c["pairs"], c["num"], c["pts"], c["att"], c["lifetime"])
     P.islands(E, O, w, o, 0)
-    P.solve(E, O, w, o, 0, STEP_TOL)
-    P.check_contacts(0, w.contacts(), o.contacts(), STEP_TOL)          # the applied impulses among them
+    # the settled pile is one island with spinning bodies in it, so every pose is in the trig set: what this holds to
+    # bits is the velocities, the applied impulses and the AABBs and inertias of the device's poses
+    g, _ = P.solve(E, O, w, o, 0)
+    P.resync(o, w, 0, g)
 
 
 # ----------------------------------------------------------------------------- free-running trajectories

@@ -2,8 +2,8 @@
 collision filters, hinges with arbitrary axes and pivots, 1-20 velocity and 0-6 position iterations) on the device, in
 lock step with the oracle, in three modes: plain launches, CUDA graphs with rebuild reuse, dataflow only.  Every step:
 the island-tile packing against its restatement (tests/tile_packing.py), ordered pair lists and island labels identical
-to the oracle's, the state within 1e-5 of the oracle replaying the device's order (at least half the steps
-bit-identical), the three modes bit-identical to each other, no error flags.  One batched world puts 32 scenes side by
+to the oracle's, the state, contacts and hinge impulses bit-identical to the oracle replaying the device's order outside
+the trig set of tests/parity.py, the three modes bit-identical to each other, no error flags.  One batched world puts 32 scenes side by
 side, so dozens of tiles and the dataflow path run at once.  Also runs against the CPU emulation (B2D_EMU=1), with fewer
 seeds and no graphs."""
 import os
@@ -12,7 +12,7 @@ import numpy as np
 import pytest
 
 from tests import tile_packing as TP
-from tests.parity import lockstep, same_digests
+from tests.parity import lockstep, report, same_digests
 from tests.test_ref_stepper import random_scene, random_scene_wide
 
 pytestmark = pytest.mark.gpu
@@ -24,15 +24,16 @@ MODES = ("plain", "dataflow") if EMU else ("plain", "graph", "dataflow")
 NARROW_ITERS = [(10, 3), (1, 0), (20, 6)]
 
 
-def _all_modes(E, O, scene, steps, min_exact=None, **kw):
-    """The lock step in every mode, at least `min_exact` steps (default half) bit-identical to the oracle; returns the
-    packing check of the plain launches."""
+def _all_modes(E, O, scene, steps, **kw):
+    """The lock step in every mode; returns the packing check of the plain launches."""
     digests, checks = {}, {}
     for mode in MODES:
         pc = checks[mode] = TP.PackingCheck(scene)
         res = lockstep(E, O, scene, steps, mode=mode, hook=pc, **kw)
         assert res["ok"], (scene["name"], mode, res)
-        assert res["exact"] >= (steps // 2 if min_exact is None else min_exact), (scene["name"], mode, res["exact"])
+        # nearly every body of these scenes spins at every step, so nearly every pose is in the trig set: what they hold
+        # to bits is the velocities, contacts, hinge impulses, AABBs and inertias (the report line gives the split)
+        report(f"{scene['name']} {mode}", res)
         assert pc.rebuilt + pc.reused == steps
         if mode == "dataflow":
             assert pc.tiled_steps == 0
@@ -79,10 +80,7 @@ def batched_random_scenes(E, O, count=32, pitch=10.0):
 
 def test_batched_random_scenes_lockstep(gpu, E, O):
     scene = batched_random_scenes(E, O, count=8 if EMU else 32)
-    # about 1 600 bodies: a step is bit-identical only if every body is, so the one-ulp residuals test_gpu_parity.py
-    # describes leave fewer exact steps than in a 46-body scene (27 of 100 on an H100); every step stays within 1e-5
-    # and the three modes must still be bit-identical to each other
-    pc = _all_modes(E, O, scene, 40 if EMU else 100, min_exact=20)
+    pc = _all_modes(E, O, scene, 40 if EMU else 100)
     # many tiles at once, and manifolds on the dataflow path in the same steps
     assert max(len(h["fill"]) for h in pc.history) >= (2 if EMU else 8), [len(h["fill"]) for h in pc.history]
     assert sum(h["dataflow"] > 0 and len(h["fill"]) > 1 for h in pc.history) >= len(pc.history) // 2, [h["dataflow"] for h in pc.history]
