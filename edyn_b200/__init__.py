@@ -8,5 +8,5 @@ from .rigidbody import (DYNAMIC, KINEMATIC, MATERIAL_NONE, MATERIAL_UNASSIGNED, 
                         capsule_shape, plane_shape, sphere_shape)
 from .world import (RAY_CAPSULE_SIDE, RAY_FEATURE_NONE, RAY_MISS, RaycastResult, World, attach,  # noqa: F401
                     clear_collision_exclusion, detach, exclude_collision, insert_material_mixing, make_hinge, make_rigidbody, raycast,
-                    remove_collision_exclusion, step_simulation, update)
+                    remove_collision_exclusion, set_paused, step_simulation, update)
 from . import scenes  # noqa: F401

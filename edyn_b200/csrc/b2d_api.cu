@@ -166,6 +166,7 @@ b2d_world *b2d_create(const b2d_config *cfg) {
     for (int k = 0; k < 3; ++k) { d.cell_org[k] = -(1 << 15); d.cell_bits[k] = 16; }
     bool ok = true;
     ok = ok && dalloc(w, d.pos, NB) && dalloc(w, d.orn, NB) && dalloc(w, d.linvel, NB) && dalloc(w, d.angvel, NB);
+    ok = ok && dalloc(w, d.ppos, NB) && dalloc(w, d.porn, NB);
     ok = ok && dalloc(w, d.matid, NB);
     d.mix_size = MIX_SLOTS;
     ok = ok && dalloc(w, d.mix_key, d.mix_size, 0xFF) && dalloc(w, d.mix_idx, d.mix_size) && dalloc(w, d.mix_mat, d.mix_size / 2);
@@ -382,6 +383,7 @@ int b2d_add_bodies(b2d_world *w, const b2d_bodies *b, uint32_t *first_id) {
         if (b->group && b->mask && !(g == ~0ULL && m == ~0ULL)) f |= F_FILTER;
         const uint32_t mid = b->material ? b->material[i] : B2D_MATERIAL_UNASSIGNED;
         if (mid == B2D_MATERIAL_NONE) f |= F_SENSOR;
+        if (b->presentation && b->presentation[i]) f |= F_PRESENT;
         matid[i] = mid == B2D_MATERIAL_NONE ? MATERIAL_UNASSIGNED : mid;
         class_add(w, sk != B2D_SHAPE_NONE ? shape_diameter(sk, b->shape_params + 4 * i) : 0.0f, dyn);
         flags[i] = f; mat[i] = make_float2(b->friction[i], b->restitution[i]); grp[i] = g; msk[i] = m;
@@ -389,6 +391,8 @@ int b2d_add_bodies(b2d_world *w, const b2d_bodies *b, uint32_t *first_id) {
     cudaStream_t s = w->stream;
     CK(cudaMemcpyAsync(d.pos + first, pos.data(), n * sizeof(float4), cudaMemcpyHostToDevice, s));
     CK(cudaMemcpyAsync(d.orn + first, orn.data(), n * sizeof(float4), cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(d.ppos + first, pos.data(), n * sizeof(float4), cudaMemcpyHostToDevice, s));     // make_rigidbody: def.position
+    CK(cudaMemcpyAsync(d.porn + first, orn.data(), n * sizeof(float4), cudaMemcpyHostToDevice, s));     // and def.orientation
     CK(cudaMemcpyAsync(d.linvel + first, lv.data(), n * sizeof(float4), cudaMemcpyHostToDevice, s));
     CK(cudaMemcpyAsync(d.angvel + first, av.data(), n * sizeof(float4), cudaMemcpyHostToDevice, s));
     CK(cudaMemcpyAsync(d.invI + 3 * (size_t)first, invI.data(), 3 * (size_t)n * sizeof(float4), cudaMemcpyHostToDevice, s));
@@ -1386,6 +1390,39 @@ int b2d_raycast_device(b2d_world *w, uint32_t n, const float *p0, const float *p
     return B2D_OK;
 }
 
+
+// ------------------------------------------------------------------ presentation (k_presentation)
+
+static int enqueue_presentation(b2d_world *w, int mode, float dt, float *out_pos, float *out_orn) {
+    cudaSetDevice(w->cfg.device);
+    Dev &d = w->d;
+    if (d.nbodies) LAUNCH(k_presentation, d.nbodies, 256, d, mode, dt, out_pos, out_orn, d.nbodies);
+    CK(cudaGetLastError());
+    return B2D_OK;
+}
+int b2d_update_presentation(b2d_world *w, float interpolation_dt) {
+    if (!w) return B2D_ERR_ARGUMENT;
+    return enqueue_presentation(w, PRESENT_UPDATE, interpolation_dt, nullptr, nullptr);
+}
+int b2d_snap_presentation(b2d_world *w) {
+    if (!w) return B2D_ERR_ARGUMENT;
+    return enqueue_presentation(w, PRESENT_SNAP, 0.0f, nullptr, nullptr);
+}
+int b2d_download_presentation(b2d_world *w, float *pos, float *orn) {
+    if (!w || (!pos && !orn)) return B2D_ERR_ARGUMENT;
+    const size_t n = w->d.nbodies;
+    float *sp = w->stage, *so = sp + 3 * n;
+    if (int rc = enqueue_presentation(w, PRESENT_READ, 0.0f, pos ? sp : nullptr, orn ? so : nullptr)) return rc;
+    cudaStream_t s = w->stream;
+    if (pos && n) CK(cudaMemcpyAsync(pos, sp, 3 * n * sizeof(float), cudaMemcpyDeviceToHost, s));
+    if (orn && n) CK(cudaMemcpyAsync(orn, so, 4 * n * sizeof(float), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    return B2D_OK;
+}
+int b2d_download_presentation_device(b2d_world *w, float *device_pos, float *device_orn) {
+    if (!w || (!device_pos && !device_orn)) return B2D_ERR_ARGUMENT;
+    return enqueue_presentation(w, PRESENT_READ, 0.0f, device_pos, device_orn);
+}
 
 int b2d_set_timing(b2d_world *w, int enabled) { if (!w) return B2D_ERR_ARGUMENT; w->timing = enabled != 0; return B2D_OK; }
 

@@ -182,10 +182,10 @@ __global__ void k_plan_constraints(Dev d, uint32_t *counts) {
 }
 
 // ---------------------------------------------------------------- hand-over blob
-// header (4 x uint4) | bodies: 11 float4 each | manifolds: 21 float4 each | hinges: 7 float4 each | exclusions: uint2 each
-// A body's flags carry F_SENSOR; its material id sits in o[10].z.
+// header (4 x uint4) | bodies: 13 float4 each | manifolds: 21 float4 each | hinges: 7 float4 each | exclusions: uint2 each
+// A body's flags carry F_SENSOR and F_PRESENT; its material id sits in o[10].z, its present transform in o[11], o[12].
 constexpr uint32_t BLOB_MAGIC = 0xB2D0B10Bu;
-constexpr uint32_t BLOB_BODY_F4 = 11, BLOB_MANIFOLD_F4 = 21, BLOB_HINGE_F4 = 7;
+constexpr uint32_t BLOB_BODY_F4 = 13, BLOB_MANIFOLD_F4 = 21, BLOB_HINGE_F4 = 7;
 struct BlobHeader { uint32_t magic, nb, nm, nh, nx; uint32_t pad[11]; };      // 64 B
 static_assert(sizeof(BlobHeader) == 64, "blob header is four 16-byte words");
 B2D_D float fbits(uint32_t u) { return __uint_as_float(u); }
@@ -209,6 +209,7 @@ __global__ void k_pack_bodies(Dev d, const uint32_t *ids, uint32_t n, float4 *ou
         o[7] = g; o[8] = d.shp[i];
         o[9] = make_float4(m.x, m.y, fbits((uint32_t)grp), fbits((uint32_t)(grp >> 32)));
         o[10] = make_float4(fbits((uint32_t)msk), fbits((uint32_t)(msk >> 32)), fbits(d.matid[i]), 0);
+        o[11] = d.ppos[i]; o[12] = d.porn[i];
     }
 }
 // flags for the deterministic compaction (slot order) of the constraints that leave for `dst`
@@ -276,6 +277,7 @@ __global__ void k_unpack_bodies(Dev d, uint32_t first, uint32_t n, const float4 
         d.group[i] = (unsigned long long)ubits(o[9].z) | ((unsigned long long)ubits(o[9].w) << 32);
         d.fmask[i] = (unsigned long long)ubits(o[10].x) | ((unsigned long long)ubits(o[10].y) << 32);
         d.matid[i] = ubits(o[10].z);
+        d.ppos[i] = o[11]; d.porn[i] = o[12];
         d.flags[i] = f;
         ehash_insert(d.ehash, d.ehash_size, d.entity[i], i);
     }

@@ -130,6 +130,39 @@ __global__ void k_pack_state(Dev d, float *pos, float *orn, float *lv, float *av
     }
 }
 
+// ====================================================================== presentation
+// update_presentation / snap_presentation (sys/update_presentation.cpp:56-93), launched between steps, never inside one.
+//   PRESENT_UPDATE  bodies with F_PRESENT that are procedural and awake: pre = pos + vel dt, pre_orn = integrate(orn, w, dt)
+//                   (the linear and angular views exclude sleeping_tag; only dynamic bodies carry procedural_tag)
+//   PRESENT_SNAP    every F_PRESENT body: pre = pos, pre_orn = orn
+//   PRESENT_READ    no write
+// out_pos / out_orn (3n / 4n floats, either may be null) receive what b2d_download_presentation reports: the present
+// transform of an F_PRESENT body, pos / orn of any other (a removed body has lost F_PRESENT).
+enum PresentMode { PRESENT_UPDATE = 0, PRESENT_SNAP = 1, PRESENT_READ = 2 };
+__global__ void k_presentation(Dev d, int mode, float dt, float *out_pos, float *out_orn, uint32_t n) {
+    GRID_STRIDE(i, n) {
+        const uint32_t f = d.flags[i];
+        const bool present = (f & F_PRESENT) != 0u;
+        float4 p, q;
+        if (present && mode == PRESENT_UPDATE && is_dynamic(f)) {
+            p = f4(mk3(d.pos[i]) + mk3(d.linvel[i]) * dt, 0.0f);
+            q = f4(integrate(mkq(d.orn[i]), mk3(d.angvel[i]), dt));
+            d.ppos[i] = p; d.porn[i] = q;
+        } else if (present && mode == PRESENT_SNAP) {
+            p = d.pos[i]; q = d.orn[i];
+            d.ppos[i] = p; d.porn[i] = q;
+        } else if (!out_pos && !out_orn) {
+            continue;
+        } else if (present) {
+            p = d.ppos[i]; q = d.porn[i];
+        } else {
+            p = d.pos[i]; q = d.orn[i];
+        }
+        if (out_pos) { out_pos[3 * i] = p.x; out_pos[3 * i + 1] = p.y; out_pos[3 * i + 2] = p.z; }
+        if (out_orn) { out_orn[4 * i] = q.x; out_orn[4 * i + 1] = q.y; out_orn[4 * i + 2] = q.z; out_orn[4 * i + 3] = q.w; }
+    }
+}
+
 // ====================================================================== broadphase
 
 constexpr float BP_OFFSET = -BREAKING_THRESHOLD;                 // m_aabb_offset, broadphase.hpp:15

@@ -16,6 +16,7 @@ constexpr uint32_t F_FILTER = 1u << 13;       // has collision_filter
 constexpr uint32_t F_LARGE = 1u << 14;        // larger than a broadphase cell: brute-force list
 constexpr uint32_t F_SLEEPING = 1u << 16;     // sleeping_tag: excluded from every per-step view until its island wakes
 constexpr uint32_t F_REMOVED = 1u << 15;      // destroyed (b2d_remove_bodies): static, shapeless, its manifolds and joints die
+constexpr uint32_t F_PRESENT = 1u << 18;      // has present_position + present_orientation (k_presentation only; no step kernel reads it)
 
 constexpr uint32_t MATERIAL_UNASSIGNED = 0xFFFFu;   // material::UnassignedID: never in the mixing table
 
@@ -208,6 +209,10 @@ struct Dev {
     uint4 *tile_hdr;
     uint4 *tplan_h, *tplan_c;
     uint2 *tplan_w;
+
+    // ---- presentation transforms (present_position xyz, present_orientation xyzw) of the F_PRESENT bodies, written by
+    // k_presentation between steps; appended last so that the step kernels' parameter offsets stay as they were
+    float4 *ppos, *porn;
 };
 
 } // namespace b2d

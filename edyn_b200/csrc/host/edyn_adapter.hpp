@@ -13,6 +13,7 @@
 // device world cannot be created.
 #pragma once
 #include "../../../include/b2d.h"
+#include <algorithm>
 #include <array>
 #include <cmath>
 #include <cstdint>
@@ -51,6 +52,7 @@ struct rigidbody_def {                               // include/edyn/util/rigidb
     std::optional<shapes_variant_t> shape;
     std::optional<edyn::material> material{edyn::material{}};
     std::uint64_t collision_group{~0ull}, collision_mask{~0ull};
+    bool presentation{true};                         // present_position / present_orientation (dynamic bodies only)
 };
 
 struct init_config {                                 // include/edyn/edyn.hpp:39-60 (+ device capacities)
@@ -69,6 +71,8 @@ class registry {
 public:
     // components, SoA (same fields the reference keeps per entity)
     std::vector<scalar> position, orientation, linvel, angvel, aabb;      // 3n, 4n, 3n, 3n, 6n
+    // present_position / present_orientation, refreshed by every update(); bodies without them hold position / orientation
+    std::vector<scalar> present_position, present_orientation;           // 3n, 4n
     std::size_t size() const { return position.size() / 3; }
 
     vector3 get_position(entity e) const { return {position[3 * e], position[3 * e + 1], position[3 * e + 2]}; }
@@ -120,6 +124,13 @@ inline void pull(registry &r) {
                   "b2d_download_state");
     (void)n;
 }
+inline void push(registry &r) {
+    if (r.dirty) { detail::check(r, b2d_upload_state(r.world, r.position.data(), r.orientation.data(), r.linvel.data(), r.angvel.data()), "b2d_upload_state"); r.dirty = false; }
+}
+inline void pull_presentation(registry &r) {
+    if (!r.size()) return;
+    detail::check(r, b2d_download_presentation(r.world, r.present_position.data(), r.present_orientation.data()), "b2d_download_presentation");
+}
 }  // namespace detail
 
 inline void attach(registry &r, const init_config &config = {}) {
@@ -158,12 +169,14 @@ inline entity make_rigidbody(registry &r, const rigidbody_def &def) {
     float fr = def.material ? def.material->friction : 0, re = def.material ? def.material->restitution : 0;
     std::uint64_t grp = def.collision_group, msk = def.collision_mask;
     std::uint32_t mat = def.material ? std::uint32_t(def.material->id) : B2D_MATERIAL_NONE;      // no material: a sensor
-    b2d_bodies b{1, pos, orn, lv, av, &inv_mass, inv_I.data(), grav, &kind, &sk, sp, &fr, &re, &grp, &msk, &mat};
+    std::uint32_t pre = def.presentation && dyn ? 1u : 0u;          // util/rigidbody.cpp:99-102
+    b2d_bodies b{1, pos, orn, lv, av, &inv_mass, inv_I.data(), grav, &kind, &sk, sp, &fr, &re, &grp, &msk, &mat, &pre};
     std::uint32_t id = 0;
     detail::check(r, b2d_add_bodies(r.world, &b, &id), "b2d_add_bodies");
     r.position.insert(r.position.end(), pos, pos + 3); r.orientation.insert(r.orientation.end(), orn, orn + 4);
     r.linvel.insert(r.linvel.end(), lv, lv + 3); r.angvel.insert(r.angvel.end(), av, av + 3);
     r.aabb.resize(r.aabb.size() + 6);
+    r.present_position.insert(r.present_position.end(), pos, pos + 3); r.present_orientation.insert(r.present_orientation.end(), orn, orn + 4);
     return id;
 }
 
@@ -211,26 +224,37 @@ inline bool is_sleeping(registry &r, entity e) {
     return asleep[e] != 0;
 }
 
-inline void set_paused(registry &r, bool paused) { r.paused = paused; }
+// edyn::set_paused (stepper_sequential.cpp:148-151): the accumulator restarts from zero
+inline void set_paused(registry &r, bool paused) { r.paused = paused; r.accumulated = 0; }
 
 // One fixed step (step_simulation semantics, stepper_sequential.cpp:121-147).
 inline void step_simulation(registry &r) {
-    if (r.dirty) { detail::check(r, b2d_upload_state(r.world, r.position.data(), r.orientation.data(), r.linvel.data(), r.angvel.data()), "b2d_upload_state"); r.dirty = false; }
+    detail::push(r);
     detail::check(r, b2d_step(r.world, 1), "b2d_step");
     detail::pull(r);
 }
 
-// edyn::update(registry, time): accumulate elapsed time, run floor(acc / fixed_dt) steps, capped (stepper_sequential.cpp:45-65).
+// edyn::update(registry, time): accumulate elapsed time, run floor(acc / fixed_dt) steps, capped (stepper_sequential.cpp:45-65),
+// then update_presentation with interpolation_dt = min(float(acc - fixed_dt), fixed_dt), the elapsed-time form of
+// stepper_sequential.cpp:104-105; while paused, snap_presentation (:37-43).  One presentation download per call.
 inline unsigned update(registry &r, double elapsed) {
-    if (r.paused) return 0;
+    detail::push(r);
+    if (r.paused) {
+        detail::check(r, b2d_snap_presentation(r.world), "b2d_snap_presentation");
+        detail::pull_presentation(r);
+        return 0;
+    }
     r.accumulated += elapsed;
     unsigned n = unsigned(std::floor(r.accumulated / r.config.fixed_dt));
     r.accumulated -= double(n) * r.config.fixed_dt;
     if (n > r.max_steps_per_update) n = r.max_steps_per_update;
-    if (!n) return 0;
-    if (r.dirty) { detail::check(r, b2d_upload_state(r.world, r.position.data(), r.orientation.data(), r.linvel.data(), r.angvel.data()), "b2d_upload_state"); r.dirty = false; }
-    detail::check(r, b2d_step(r.world, n), "b2d_step");
-    detail::pull(r);
+    if (n) {
+        detail::check(r, b2d_step(r.world, n), "b2d_step");
+        detail::pull(r);
+    }
+    const float dt = std::min(float(r.accumulated - double(r.config.fixed_dt)), float(r.config.fixed_dt));
+    detail::check(r, b2d_update_presentation(r.world, dt), "b2d_update_presentation");
+    detail::pull_presentation(r);
     return n;
 }
 

@@ -23,6 +23,8 @@
 #include <edyn/comp/material.hpp>
 #include <edyn/comp/orientation.hpp>
 #include <edyn/comp/position.hpp>
+#include <edyn/comp/present_orientation.hpp>
+#include <edyn/comp/present_position.hpp>
 #include <edyn/comp/shape_index.hpp>
 #include <edyn/comp/tag.hpp>
 #include <edyn/constraints/hinge_constraint.hpp>
@@ -32,6 +34,7 @@
 #include <edyn/util/visit_component.hpp>
 #include "b2d.h"
 #include <algorithm>
+#include <cmath>
 #include <cstdint>
 #include <stdexcept>
 #include <string>
@@ -47,6 +50,13 @@ extern "C" {
 int b2d_set_material_mixing(b2d_world *w, uint32_t n, const uint32_t *id0, const uint32_t *id1, const float *friction,
                             const float *restitution) __attribute__((weak));
 int b2d_remove_material_mixing(b2d_world *w, uint32_t n, const uint32_t *id0, const uint32_t *id1) __attribute__((weak));
+}
+// So are the presentation entry points: update() calls them only once a staged body has present_position /
+// present_orientation, and throws then if the linked libb2d lacks them.
+extern "C" {
+int b2d_update_presentation(b2d_world *w, float interpolation_dt) __attribute__((weak));
+int b2d_snap_presentation(b2d_world *w) __attribute__((weak));
+int b2d_download_presentation(b2d_world *w, float *pos3n, float *orn4n) __attribute__((weak));
 }
 
 namespace edyn {
@@ -74,9 +84,12 @@ class stepper_b2d {
     std::vector<uint32_t> m_asleep, m_was_asleep;            // B2D_FLAG_SLEEPING: sleeping_tag per body, this step / last step
     bool m_sleeping {false};
     std::vector<float> m_pos, m_orn, m_lv, m_av, m_aabb;     // download buffers
+    std::vector<float> m_ppos, m_porn;                       // presentation download buffers
     std::unordered_map<uint64_t, entt::entity> m_manifold_of;   // (body id 0 << 32 | body id 1) -> mirrored contact_manifold entity
     uint64_t m_steps {0}, m_mirror_step {0};
     double m_last_time;
+    double m_accumulated_time {};                            // stepper_sequential::m_accumulated_time
+    bool m_presentation {false};                             // a staged body has present_position / present_orientation
     bool m_paused {false};
     bool m_scattering {false};                               // our own component writes are not "dirty"
 
@@ -190,8 +203,13 @@ public:
         std::vector<uint32_t> kind(n), sk(n);
         std::vector<uint64_t> grp(n, ~0ull), msk(n, ~0ull);
         std::vector<uint32_t> mid(n, B2D_MATERIAL_NONE);                    // no material component: a sensor
+        std::vector<uint32_t> pre(n, 0u);
         for (uint32_t i = 0; i < n; ++i) {
             const auto e = m_new_bodies[i];
+            const bool has_pp = reg.all_of<present_position>(e), has_po = reg.all_of<present_orientation>(e);
+            if (has_pp != has_po) throw std::runtime_error("stepper_b2d: a body with only one of present_position and present_orientation is not supported");
+            pre[i] = has_pp ? 1u : 0u;
+            m_presentation |= has_pp;
             put3(&pos[3 * i], reg.get<position>(e));
             const auto &q = reg.get<orientation>(e);
             orn[4 * i] = float(q.x); orn[4 * i + 1] = float(q.y); orn[4 * i + 2] = float(q.z); orn[4 * i + 3] = float(q.w);
@@ -220,7 +238,7 @@ public:
             if (auto *f = reg.try_get<collision_filter>(e)) { grp[i] = f->group; msk[i] = f->mask; }
         }
         b2d_bodies b {n, pos.data(), orn.data(), lv.data(), av.data(), im.data(), iI.data(), g.data(), kind.data(), sk.data(), sp.data(),
-                      fr.data(), re.data(), grp.data(), msk.data(), mid.data()};
+                      fr.data(), re.data(), grp.data(), msk.data(), mid.data(), pre.data()};
         uint32_t first = 0;
         check(b2d_add_bodies(m_world, &b, &first), "b2d_add_bodies");
         for (uint32_t i = 0; i < n; ++i) {
@@ -401,6 +419,32 @@ public:
         m_scattering = false;
     }
 
+    // ---- device -> registry: present_position / present_orientation after b2d_update_presentation or b2d_snap_presentation,
+    // written in place without signals, like update_presentation does
+    // b2d_snap_presentation or b2d_update_presentation, then the components; nothing while no body has presentation
+    void present(bool snap, float interpolation_dt) {
+        if (!m_presentation) return;
+        if (!b2d_update_presentation || !b2d_snap_presentation || !b2d_download_presentation)
+            throw std::runtime_error("stepper_b2d: the linked libb2d has no presentation transforms (b2d_update_presentation)");
+        if (snap) check(b2d_snap_presentation(m_world), "b2d_snap_presentation");
+        else check(b2d_update_presentation(m_world, interpolation_dt), "b2d_update_presentation");
+        scatter_presentation();
+    }
+    void scatter_presentation() {
+        auto &reg = *m_registry;
+        const auto n = m_entities.size();
+        m_ppos.resize(3 * n); m_porn.resize(4 * n);
+        if (n) check(b2d_download_presentation(m_world, m_ppos.data(), m_porn.data()), "b2d_download_presentation");
+        auto view = reg.view<present_position, present_orientation>();
+        for (size_t i = 0; i < n; ++i) {
+            const auto e = m_entities[i];
+            if (e == entt::null || !view.contains(e)) continue;
+            auto [p, q] = view.get(e);
+            p.x = m_ppos[3 * i]; p.y = m_ppos[3 * i + 1]; p.z = m_ppos[3 * i + 2];
+            q.x = m_porn[4 * i]; q.y = m_porn[4 * i + 1]; q.z = m_porn[4 * i + 2]; q.w = m_porn[4 * i + 3];
+        }
+    }
+
     // sleeping_tag on the bodies as island_manager::put_to_sleep / wake_up_island leave it (island_manager.cpp:541-566,
     // :257-295); islands fall asleep and wake up on the device
     void sync_sleeping() {
@@ -424,33 +468,57 @@ public:
         if (id < m_was_asleep.size()) m_was_asleep[id] = 0;
     }
 
-    // ---- stepper_sequential's public surface
-    void step_simulation(double time) {                                // stepper_sequential.cpp:121-147 (one fixed step)
-        auto &s = m_registry->ctx().get<settings>();
+    // everything the user changed in the registry since the last call travels to the device
+    void stage() {
         check_material_toggles();
         stage_new_bodies();
         stage_new_hinges();
         stage_exclusions();
         upload_dirty();
         sync_material_table();
+    }
+
+    void step_once() {
+        auto &s = m_registry->ctx().get<settings>();
+        stage();
         if (s.pre_step_callback) (*s.pre_step_callback)(*m_registry);
         check(b2d_step(m_world, 1), "b2d_step");
         ++m_steps;
         scatter_state();                                               // blocks until the step's results are on the host
         if (m_sleeping) sync_sleeping();
         if (s.post_step_callback) (*s.post_step_callback)(*m_registry);
-        m_last_time = time;
     }
 
-    void update(double time) {                                         // stepper_sequential.cpp:28-69: the fixed-step accumulator
-        if (m_paused) { m_last_time = time; return; }
+    // ---- stepper_sequential's public surface
+    void step_simulation(double time) {                                // stepper_sequential.cpp:121-147 (one fixed step)
+        m_last_time = time;
+        step_once();
+    }
+
+    // stepper_sequential.cpp:28-69, :104-105: the fixed-step accumulator, then the presentation transforms.  Time beyond
+    // max_steps_per_update fixed steps is dropped, as the reference drops it.  While paused only snap_presentation runs and
+    // the last time stays where it was (:37-43).
+    void update(double time) {
+        if (m_paused) {
+            stage();
+            present(true, 0.0f);
+            return;
+        }
         const auto &s = m_registry->ctx().get<settings>();
-        const double fixed_dt = double(s.fixed_dt);
-        const double elapsed = std::min(time - m_last_time, double(s.max_steps_per_update) * fixed_dt);
-        const int num_steps = int(elapsed / fixed_dt);
-        const double start = m_last_time;
-        for (int i = 0; i < num_steps; ++i) step_simulation(start + double(i + 1) * fixed_dt);
-        m_last_time = start + double(num_steps) * fixed_dt;
+        const auto elapsed = std::max(time - m_last_time, 0.0);
+        m_accumulated_time += elapsed;
+        const auto fixed_dt = s.fixed_dt;
+        const auto num_steps = static_cast<uint64_t>(std::floor(m_accumulated_time / fixed_dt));
+        const auto advance_dt = static_cast<double>(num_steps) * fixed_dt;
+        m_accumulated_time -= advance_dt;
+        const auto effective_steps = std::min<uint64_t>(num_steps, s.max_steps_per_update);
+        for (uint64_t i = 0; i < effective_steps; ++i) step_once();
+        m_last_time = time;
+        // update_presentation(registry, get_simulation_timestamp(), time, elapsed, fixed_dt), update_presentation.cpp:70
+        const double sim_time = m_last_time - m_accumulated_time;
+        const auto interpolation_dt = std::min(static_cast<scalar>(time - double(fixed_dt) - sim_time), s.fixed_dt);
+        stage();                                                       // bodies created or patched since the last step count too
+        present(false, float(interpolation_dt));
     }
 
     // ---- contacts, on demand (SURVEY.md section 8 f2).  The device keeps manifolds and points resident; creating and
@@ -558,7 +626,7 @@ private:
     }
 
 public:
-    void set_paused(bool paused) { m_paused = paused; }
+    void set_paused(bool paused) { m_paused = paused; m_accumulated_time = 0; }       // stepper_sequential.cpp:148-151
     bool is_paused() const { return m_paused; }
 };
 

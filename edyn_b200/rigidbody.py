@@ -62,6 +62,7 @@ class RigidBodyDef:                    # include/edyn/util/rigidbody.hpp rigidbo
     material: Optional[Material] = field(default_factory=Material)     # None: a sensor (collides, is never pushed)
     collision_group: int = 0xFFFFFFFFFFFFFFFF
     collision_mask: int = 0xFFFFFFFFFFFFFFFF
+    presentation: bool = True          # present_position / present_orientation; make_rigidbody emplaces them on dynamic bodies only
 
 
 def moment_of_inertia(shape: Shape, mass) -> np.ndarray:
@@ -128,7 +129,7 @@ def bodies_soa(defs: Sequence[RigidBodyDef], default_gravity=(0.0, -9.8, 0.0)) -
                gravity=np.zeros((n, 3), f32), kind=np.zeros(n, np.uint32), shape_kind=np.full(n, SHAPE_NONE, np.uint32),
                shape_params=np.zeros((n, 4), f32), friction=np.zeros(n, f32), restitution=np.zeros(n, f32),
                group=np.full(n, 0xFFFFFFFFFFFFFFFF, np.uint64), mask=np.full(n, 0xFFFFFFFFFFFFFFFF, np.uint64),
-               material=np.full(n, MATERIAL_UNASSIGNED, np.uint32))
+               material=np.full(n, MATERIAL_UNASSIGNED, np.uint32), presentation=np.zeros(n, np.uint32))
     cache = {}
     for i, d in enumerate(defs):
         out["pos"][i] = d.position
@@ -160,4 +161,5 @@ def bodies_soa(defs: Sequence[RigidBodyDef], default_gravity=(0.0, -9.8, 0.0)) -
             out["material"][i] = MATERIAL_NONE
         out["group"][i] = d.collision_group
         out["mask"][i] = d.collision_mask
+        out["presentation"][i] = 1 if d.presentation and d.kind == DYNAMIC else 0
     return out

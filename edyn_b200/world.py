@@ -8,7 +8,8 @@ Mirrors the reference's lifecycle surface for the sequential stepper
     exclude_collision(world, a, b)    edyn::exclude_collision
     insert_material_mixing(world, id0, id1, material)   edyn::insert_material_mixing
     step_simulation(world)            edyn::step_simulation(registry, t)   (one fixed step)
-    update(world, dt_elapsed)         edyn::update(registry, time)         (accumulator, <= max_steps)
+    update(world, dt_elapsed)         edyn::update(registry, time)         (accumulator, <= max_steps, presentation)
+    set_paused(world, paused)         edyn::set_paused
     set_solver_velocity_iterations... edyn::set_solver_velocity_iterations
 All compute happens in libb2d.so on the GPU; nothing here touches oracle/.
 """
@@ -65,6 +66,7 @@ class World:
         self.max_manifolds = max_manifolds
         self._accum = 0.0
         self.max_steps_per_update = 10          # settings.max_steps_per_update
+        self.paused = False                     # settings.paused
 
     # -- lifecycle
     def close(self):
@@ -94,9 +96,10 @@ class World:
         grp = _c(soa["group"], np.uint64, (n,)) if soa.get("group") is not None else None
         msk = _c(soa["mask"], np.uint64, (n,)) if soa.get("mask") is not None else None
         mat = _c(soa["material"], u32, (n,)) if soa.get("material") is not None else None     # absent: all unassigned
+        pre = _c(soa["presentation"], u32, (n,)) if soa.get("presentation") is not None else None     # absent: none
         b = Bodies(n, *[_p(keep[k]) for k in ("pos", "orn", "linvel", "angvel", "inv_mass", "inv_inertia", "gravity",
                                                "kind", "shape_kind", "shape_params", "friction", "restitution")],
-                   _p(grp), _p(msk), _p(mat))
+                   _p(grp), _p(msk), _p(mat), _p(pre))
         first = C.c_uint32(0)
         self._check(self.l.b2d_add_bodies(self.h, C.byref(b), C.byref(first)))
         self.num_bodies += n
@@ -105,6 +108,7 @@ class World:
         keep["mask"] = msk if msk is not None else np.full(n, ~np.uint64(0), np.uint64)
         keep["has_filter"] = np.full(n, grp is not None and msk is not None, bool)
         keep["material"] = mat if mat is not None else np.full(n, MATERIAL_UNASSIGNED, u32)
+        keep["presentation"] = pre if pre is not None else np.zeros(n, u32)
         self._defs.append(keep)
         return first.value
 
@@ -281,6 +285,29 @@ class World:
         self._check(self.l.b2d_download_hinge_impulses(self.h, _p(imp)))
         return imp[:self.num_hinges]
 
+    # -- presentation transforms (include/b2d.h, b2d_update_presentation: semantics)
+    def update_presentation(self, interpolation_dt):
+        """update_presentation: present transforms of the awake dynamic bodies with presentation = state extrapolated
+        by interpolation_dt seconds (enqueued on the world's stream)."""
+        self._check(self.l.b2d_update_presentation(self.h, C.c_float(interpolation_dt)))
+
+    def snap_presentation(self):
+        """snap_presentation: present transforms = position / orientation for every body with presentation."""
+        self._check(self.l.b2d_snap_presentation(self.h))
+
+    def presentation(self):
+        """(present_position (n, 3), present_orientation (n, 4)) float32; bodies without presentation report their
+        position / orientation."""
+        n = self.num_bodies
+        pos, orn = np.zeros((max(1, n), 3), f32), np.zeros((max(1, n), 4), f32)
+        self._check(self.l.b2d_download_presentation(self.h, _p(pos), _p(orn)))
+        return pos[:n], orn[:n]
+
+    def presentation_device(self, pos_ptr, orn_ptr):
+        """Enqueue the copy of presentation() into integer DEVICE addresses (n x 3 and n x 4 float32; 0 = skip that one)."""
+        v = lambda x: C.c_void_p(x or None)       # noqa: E731
+        self._check(self.l.b2d_download_presentation_device(self.h, v(pos_ptr), v(orn_ptr)))
+
     # -- queries (include/b2d.h, b2d_raycast: semantics)
     def raycast(self, p0, p1, ignore=None, ignore_body=None) -> dict:
         """edyn::raycast for n segments at once: p0, p1 are (n, 3).  ignore: body ids no segment may hit; ignore_body: one id
@@ -454,13 +481,29 @@ def step_simulation(world: World):
     world.step(1)
 
 
+def set_paused(world: World, paused: bool):
+    """edyn::set_paused (stepper_sequential.cpp:148-151): the accumulator restarts from zero."""
+    world.paused = bool(paused)
+    world._accum = 0.0
+
+
 def update(world: World, elapsed: float) -> int:
     """edyn::update(registry, time): accumulate wall time, run floor(acc / fixed_dt) steps capped by
-    max_steps_per_update (stepper_sequential.cpp:45-65).  Returns the number of steps taken."""
+    max_steps_per_update (stepper_sequential.cpp:45-65), then update_presentation (:104-105).  While paused it only snaps
+    the presentation (:37-43).  Returns the number of steps taken.
+
+    The reference's interpolation_dt = min(float(time - fixed_dt - sim_time), fixed_dt) with sim_time = time - acc;
+    with elapsed times instead of timestamps that is min(float(acc - fixed_dt), fixed_dt): the present transforms lag
+    one fixed step behind the wall clock, so that frames between two steps move smoothly."""
+    if world.paused:
+        world.snap_presentation()
+        return 0
     world._accum += elapsed
     n = int(world._accum / world.fixed_dt)
     world._accum -= n * world.fixed_dt
     n = min(n, world.max_steps_per_update)
     if n:
         world.step(n)
+    fixed_dt = f32(world.fixed_dt)
+    world.update_presentation(min(f32(world._accum - float(fixed_dt)), fixed_dt))
     return n

@@ -92,7 +92,11 @@ typedef struct b2d_config {
  *   B2D_MATERIAL_NONE: an empty rigidbody_def::material, a sensor (util/collision_util.cpp:358-384,
  *   util/constraint_util.cpp:82-85).  A sensor's pairs get manifolds and contact points like any other pair, join and keep
  *   awake islands like them, but get no contact constraint: nothing pushes or bounces on a sensor, and its friction and
- *   restitution are not read.  Other values: B2D_ERR_ARGUMENT. */
+ *   restitution are not read.  Other values: B2D_ERR_ARGUMENT.
+ * presentation: n values or NULL (= none).  Non-zero: the body has present_position and present_orientation
+ *   (rigidbody_def::presentation, util/rigidbody.cpp:99-102), both starting at pos / orn.  make_rigidbody emplaces them on
+ *   dynamic bodies only; a non-zero value on a kinematic or static body is accepted and that body is snapped by
+ *   b2d_snap_presentation but never interpolated, as the reference's views would treat it. */
 typedef struct b2d_bodies {
     uint32_t count;
     const float *pos;          /* 3n  position */
@@ -110,6 +114,7 @@ typedef struct b2d_bodies {
     const uint64_t *group;     /* n or NULL  collision_filter.group */
     const uint64_t *mask;      /* n or NULL  collision_filter.mask */
     const uint32_t *material;  /* n or NULL  material.id, B2D_MATERIAL_UNASSIGNED or B2D_MATERIAL_NONE (sensor) */
+    const uint32_t *presentation; /* n or NULL  has present_position / present_orientation */
 } b2d_bodies;
 
 /* profile_counters + profile_timers analogue (include/edyn/context/profile.hpp:8-27). */
@@ -298,6 +303,27 @@ int b2d_raycast(b2d_world *w, uint32_t n, const float *p0, const float *p1, cons
 int b2d_raycast_device(b2d_world *w, uint32_t n, const float *p0, const float *p1, const uint32_t *ignore_body,
                        const uint32_t *ignore_list, uint32_t nignore, uint32_t *body, float *fraction, float *normal,
                        uint32_t *feature);
+
+/* ---- Presentation transforms: update_presentation / snap_presentation (src/edyn/sys/update_presentation.cpp:56-93), which
+ * stepper_sequential::update runs after its steps (src/edyn/simulation/stepper_sequential.cpp:37-43, :104-105).  Only bodies
+ * added with a non-zero b2d_bodies.presentation have the two components; they live on the device next to the state.
+ *   b2d_update_presentation  for every body with presentation that is dynamic and not sleeping:
+ *                            present_position = pos + linvel * interpolation_dt,
+ *                            present_orientation = integrate(orn, angvel, interpolation_dt) (math/quaternion.cpp:7-22).
+ *                            The caller computes interpolation_dt as the reference does: min(float(time - fixed_dt -
+ *                            sim_time), fixed_dt), usually negative.  Sleeping, kinematic and static bodies keep theirs.
+ *   b2d_snap_presentation    for every body with presentation: present_position = pos, present_orientation = orn (what
+ *                            update() does while paused).
+ * Both only enqueue work on b2d_stream(w); no step reads or writes the presentation.
+ *   b2d_download_presentation         pos3n / orn4n: HOST arrays (either may be NULL, not both); returns when they are filled.
+ *   b2d_download_presentation_device  the same into DEVICE pointers (e.g. a graphics-interop buffer the caller
+ *                                     owns); only enqueues on b2d_stream(w).
+ * In both downloads a body without presentation reports its current pos / orn, and a removed body what
+ * b2d_download_state reports for it. */
+int b2d_update_presentation(b2d_world *w, float interpolation_dt);
+int b2d_snap_presentation(b2d_world *w);
+int b2d_download_presentation(b2d_world *w, float *pos3n, float *orn4n);
+int b2d_download_presentation_device(b2d_world *w, float *device_pos3n, float *device_orn4n);
 
 /* Per-kernel CUDA-event timing of the velocity solve and the integrator (b2d_get_stats).  On (default): a step is
  * replayed as three CUDA graphs with the events in between; off: as one graph. */
