@@ -177,6 +177,11 @@ b2d_world *b2d_create(const b2d_config *cfg) {
     ok = ok && dalloc(w, d.bprec_min, NB) && dalloc(w, d.bprec_max, NB) && dalloc(w, d.cell_box, 6);
     d.chash_size = pow2_at_least(2ull * NB);
     ok = ok && dalloc(w, d.chash_key, d.chash_size, 0xFF) && dalloc(w, d.chash_val, d.chash_size);
+    // direct cell table: DENSE_CELLS_PER_BODY cells per body; B2D_BP_CELL_TABLE overrides the factor (0: the cell hash on every step)
+    uint64_t cells_per_body = DENSE_CELLS_PER_BODY;
+    if (const char *e = getenv("B2D_BP_CELL_TABLE")) cells_per_body = (uint64_t)std::max(0, atoi(e));
+    d.cstart_size = (uint32_t)std::min<uint64_t>(cells_per_body * NB, 0xFFFFFFFFull);
+    ok = ok && dalloc(w, d.cstart, d.cstart_size, 0xFF);
     ok = ok && dalloc(w, d.large_list, NB) && dalloc(w, d.newcount, NB) && dalloc(w, d.newoff, NB) && dalloc(w, d.newpairs, NM);
     ok = ok && dalloc(w, d.free_flag, NM) && dalloc(w, d.free_rank, NM) && dalloc(w, d.free_list, NM);
     d.mhash_size = pow2_at_least(2ull * NM);
@@ -630,7 +635,6 @@ int b2d_remove_material_mixing(b2d_world *w, uint32_t n, const uint32_t *id0, co
 static int enqueue_broadphase(b2d_world *w) {
     Dev &d = w->d; cudaStream_t s = w->stream;
     CK(cudaMemsetAsync(d.mhash_key, 0xFF, (size_t)d.mhash_size * sizeof(unsigned long long), s));
-    CK(cudaMemsetAsync(d.chash_key, 0xFF, (size_t)d.chash_size * sizeof(unsigned long long), s));
     LAUNCH(k_bp_separate, d.NM, 256, d);
     size_t t = w->cub_tmp_bytes;
     CK(cub::DeviceScan::ExclusiveSum(w->cub_tmp, t, d.free_flag, d.free_rank, (int)d.NM, s)); ++w->launches;
@@ -638,6 +642,7 @@ static int enqueue_broadphase(b2d_world *w) {
     if (d.nbodies) {
         CK(cudaMemsetAsync(d.cell_box, 0xFF, 6 * sizeof(uint32_t), s));
         LAUNCH(k_bp_cells, d.nbodies, 256, d, d.cellkey, d.cellbody, d.cell_box);
+        LAUNCH(k_bp_cell_mode, d.chash_size, 256, d);            // direct table or cell hash (clears the hash when it is used)
         t = w->cub_tmp_bytes;
         CK(cub::DeviceRadixSort::SortPairs(w->cub_tmp, t, d.cellkey, d.cellkey_s, d.cellbody, d.cellbody_s, (int)d.nbodies, 0, w->cell_key_bits, s)); w->launches += 4;
         LAUNCH(k_bp_cell_starts, d.nbodies, 256, d);

@@ -246,6 +246,27 @@ B2D_D CellBox load_cell_box(const Dev &d) {
 B2D_D bool in_cell_box(const CellBox &b, CellFields f) {
     return f.x >= b.lo[0] && f.x <= b.hi[0] && f.y >= b.lo[1] && f.y <= b.hi[1] && f.z >= b.lo[2] && f.z <= b.hi[2];
 }
+B2D_D CellFields key_fields(const Dev &d, unsigned long long k) {
+    const uint32_t by = d.cell_bits[1], bz = d.cell_bits[2];
+    return CellFields{(uint32_t)(k >> (by + bz)), (uint32_t)(k >> bz) & ((1u << by) - 1u), (uint32_t)k & ((1u << bz) - 1u)};
+}
+// Direct cell table (Dev::cstart): a cell of the box at its fields minus the box's low corner, linearised with z fastest,
+// so the three cells of a column are adjacent words.  Only valid when the box has at most d.cstart_size cells.
+B2D_D uint32_t cell_index(const CellBox &b, CellFields f) {
+    return ((f.x - b.lo[0]) * (b.hi[1] - b.lo[1] + 1u) + (f.y - b.lo[1])) * (b.hi[2] - b.lo[2] + 1u) + (f.z - b.lo[2]);
+}
+// The first sorted index of an occupied cell of the box, or false.  Direct mode: k_bp_cell_starts stores the run head of
+// every cell occupied this step, over whatever the entry held.  The table is never cleared, so the entry of a cell that
+// is empty this step may be left from an earlier step, or from an earlier box (another linearisation), or be the
+// allocation's fill.  No body has that cell's key this step, so such an entry fails `e < nbodies && cellkey_s[e] ==
+// key` whatever index it holds.  Hash mode: the cell hash, cleared and filled this step.
+B2D_D bool cell_find(const Dev &d, const CellBox &b, bool direct, CellFields f, unsigned long long key, uint32_t &start) {
+    if (!direct) return hash_find(d.chash_key, d.chash_val, d.chash_size, key, start);
+    const uint32_t e = d.cstart[cell_index(b, f)];
+    if (e >= d.nbodies || d.cellkey_s[e] != key) return false;
+    start = e;
+    return true;
+}
 B2D_D void cell_of(const Dev &d, float4 a, float4 b, int &cx, int &cy, int &cz) {
     cx = (int)floorf((a.x + b.x) * 0.5f * d.inv_cell);
     cy = (int)floorf((a.y + b.y) * 0.5f * d.inv_cell);
@@ -282,6 +303,18 @@ __global__ void k_bp_cells(Dev d, unsigned long long *cellkey, uint32_t *cellbod
     __syncthreads();
     if (threadIdx.x < 6 && sm[threadIdx.x] != ~0u) atomicMin(&box[threadIdx.x], sm[threadIdx.x]);
 }
+// After k_bp_cells: this step's cell lookup.  The direct table when the occupied box has no more cells than it (an empty
+// box has none), the cell hash otherwise (sparse worlds); only then is the hash cleared, here, for k_bp_cell_starts.
+__global__ void k_bp_cell_mode(Dev d) {
+    const CellBox b = load_cell_box(d);
+    unsigned long long cells = 1;
+    #pragma unroll
+    for (int k = 0; k < 3; ++k) cells *= b.hi[k] >= b.lo[k] ? (unsigned long long)(b.hi[k] - b.lo[k]) + 1ull : 0ull;
+    const bool direct = cells <= d.cstart_size;
+    if (blockIdx.x == 0 && threadIdx.x == 0) d.cnt->bp_direct = direct;
+    if (direct) return;
+    GRID_STRIDE(k, d.chash_size) d.chash_key[k] = EMPTY_KEY;
+}
 // Cells occupied by the bodies that go into the grid (host: sizes the key fields, b2d_api.cu measure_cells)
 __global__ void k_cell_extent(Dev d, int *out6) {
     int mn[3] = {0x7FFFFFFF, 0x7FFFFFFF, 0x7FFFFFFF}, mx[3] = {-0x7FFFFFFF, -0x7FFFFFFF, -0x7FFFFFFF};
@@ -309,10 +342,12 @@ B2D_D uint32_t key_body(const Dev &d, uint2 pr) {
 }
 // spatial part of a dataflow manifold's sort key (k_color_keys): the key body's rank in the cell order, 14 bits
 B2D_D uint32_t df_spatial(const Dev &d, uint32_t rank) { return (uint32_t)(((unsigned long long)rank << KEY_DF_SPATIAL_BITS) / d.nbodies); }
-// First sorted index of every occupied cell -> hash table, and every body's candidate record in the sorted order (what
-// bp_candidate reads about it), so the neighbourhood search walks records instead of gathering by body id.  A body that
-// is not in an island tile and whose spatial rank moved would change a dataflow sort key: the island rebuild has to run.
+// First sorted index of every occupied cell -> the direct table (a plain store: one run head per cell) or the cell hash,
+// as k_bp_cell_mode chose, and every body's candidate record in the sorted order (what bp_candidate reads about it), so
+// the neighbourhood search walks records instead of gathering by body id.  A body that is not in an island tile and
+// whose spatial rank moved would change a dataflow sort key: the island rebuild has to run.
 __global__ void k_bp_cell_starts(Dev d) {
+    const bool direct = d.cnt->bp_direct;
     GRID_STRIDE(i, d.nbodies) {
         // the gathers first: they are independent of each other and of the hash insert's atomics
         const uint32_t b = d.cellbody_s[i];
@@ -320,7 +355,10 @@ __global__ void k_bp_cell_starts(Dev d) {
         d.bprec_min[i] = make_float4(mn.x, mn.y, mn.z, __uint_as_float(b));
         d.bprec_max[i] = make_float4(mx.x, mx.y, mx.z, __uint_as_float(d.flags[b]));
         unsigned long long k = d.cellkey_s[i];
-        if (k != EMPTY_KEY && (i == 0 || d.cellkey_s[i - 1] != k)) hash_insert(d.chash_key, d.chash_val, d.chash_size, k, i);
+        if (k != EMPTY_KEY && (i == 0 || d.cellkey_s[i - 1] != k)) {
+            if (direct) d.cstart[cell_index(load_cell_box(d), key_fields(d, k))] = i;
+            else hash_insert(d.chash_key, d.chash_val, d.chash_size, k, i);
+        }
         if (df_spatial(d, d.brank[b]) != df_spatial(d, i) && d.btile[b] == TILE_NONE) d.cnt->graph_changed = 1u;
         d.brank[b] = i;
     }
@@ -381,13 +419,14 @@ B2D_D void bp_candidate_rec(const Dev &d, uint32_t A, uint32_t fA, const box3 &b
 // order of a probe and a walk per cell.  Where cell_key_of clamps z (outside the extent measured at capture), two or
 // three offsets share a key; only the first of them is probed, so the cell is walked once and each pair found once.
 struct BpColumn { unsigned long long key[3]; uint32_t start[3]; bool occ[3]; };
-B2D_D BpColumn bp_column_find(const Dev &d, const CellBox &box, int x, int y, int cz) {
+// In direct mode the column's cells are adjacent words of the table.
+B2D_D BpColumn bp_column_find(const Dev &d, const CellBox &box, bool direct, int x, int y, int cz) {
     BpColumn c;
     #pragma unroll
     for (int z = 0; z < 3; ++z) {
         const CellFields f = cell_fields(d, x, y, cz + z - 1);
         c.key[z] = cell_key(d, f);
-        c.occ[z] = (z == 0 || c.key[z] != c.key[z - 1]) && in_cell_box(box, f) && hash_find(d.chash_key, d.chash_val, d.chash_size, c.key[z], c.start[z]);
+        c.occ[z] = (z == 0 || c.key[z] != c.key[z - 1]) && in_cell_box(box, f) && cell_find(d, box, direct, f, c.key[z], c.start[z]);
     }
     return c;
 }
@@ -405,7 +444,8 @@ B2D_D void bp_column_walk(const Dev &d, const BpColumn &c, uint32_t A, uint32_t 
 }
 
 template<bool FILL>
-__global__ void k_bp_pairs(Dev d) {
+// (launch bounds: at most 56 registers, nine CTAs of 128 per SM, the residency the search had before the direct table)
+__global__ void __launch_bounds__(128, 9) k_bp_pairs(Dev d) {
     GRID_STRIDE(t, d.nbodies) {
         // threads walk the bodies in cell order: a warp's queries hit the same cells and candidate records (output
         // slots are still indexed by body id, so the pair order does not change)
@@ -426,11 +466,12 @@ __global__ void k_bp_pairs(Dev d) {
             if (!(fA & F_LARGE)) {
                 int cx, cy, cz; cell_of(d, rmn, rmx, cx, cy, cz);
                 const CellBox box = load_cell_box(d);
+                const bool direct = d.cnt->bp_direct;
                 for (int dx = -1; dx <= 1; ++dx) {
                     if (dx > -1 && cell_field(d, 0, cx + dx) == cell_field(d, 0, cx + dx - 1)) continue;      // clamped: same cells
                     for (int dy = -1; dy <= 1; ++dy) {
                         if (dy > -1 && cell_field(d, 1, cy + dy) == cell_field(d, 1, cy + dy - 1)) continue;
-                        bp_column_walk(d, bp_column_find(d, box, cx + dx, cy + dy, cz), A, fA, bbA, qA, count, out);
+                        bp_column_walk(d, bp_column_find(d, box, direct, cx + dx, cy + dy, cz), A, fA, bbA, qA, count, out);
                     }
                 }
             } else {
@@ -476,7 +517,8 @@ __global__ void __launch_bounds__(256, FILL ? 5 : 8) k_bp_pairs_warp(Dev d) {
                     // a lane whose field repeats the previous offset's on some axis has the same cell as an earlier lane
                     const bool repeat = (ox && f.x == cell_field(d, 0, cx + ox - 2)) || (oy && f.y == cell_field(d, 1, cy + oy - 2)) ||
                                         (oz && f.z == cell_field(d, 2, cz + oz - 2));
-                    if (!repeat && in_cell_box(load_cell_box(d), f) && hash_find(d.chash_key, d.chash_val, d.chash_size, key, start)) mode = 1;
+                    const CellBox box = load_cell_box(d);
+                    if (!repeat && in_cell_box(box, f) && cell_find(d, box, d.cnt->bp_direct, f, key, start)) mode = 1;
                 }
             } else if (lane < 27u) {
                 const uint32_t chunk = (d.nbodies + 26u) / 27u;

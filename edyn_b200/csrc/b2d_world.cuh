@@ -46,6 +46,8 @@ constexpr uint32_t KEY_INACTIVE = 1u << (KEY_TILE_BITS + 7);
 constexpr int COLOR_KEY_BITS = KEY_TILE_BITS + 8;
 constexpr int KEY_DF_SPATIAL_BITS = 14;
 constexpr int KEY_DF_COLOR_SHIFT = KEY_DF_SPATIAL_BITS + 2;
+// broadphase: cells of the direct cell table per body (Dev::cstart); an occupied box with more cells uses the cell hash
+constexpr uint32_t DENSE_CELLS_PER_BODY = 4;
 
 constexpr uint32_t ERR_MANIFOLD_CAPACITY = 1u;
 constexpr uint32_t ERR_COLOR_OVERFLOW = 2u;
@@ -87,6 +89,7 @@ struct Counters {
     uint32_t graph_changed;
     unsigned long long steps_rebuilt, steps_reused;          // graph steps that ran / skipped the rebuild (statistics)
     unsigned long long dbg[16];  // development counters (B2D_DF_PROFILE builds only)
+    uint32_t bp_direct;          // this step's cell lookup: 1 the direct table (Dev::cstart), 0 the cell hash (k_bp_cell_mode)
 };
 
 struct Dev {
@@ -126,6 +129,7 @@ struct Dev {
     uint32_t *tile_nb, *tile_body;       // per tile: bodies, slot -> body (TILE_CAP per tile)
     uint32_t *tile_c0, *tile_c1, *tile_h0, *tile_h1;   // per tile: its range of the sorted contact / hinge arrays
     unsigned long long *chash_key; uint32_t *chash_val; uint32_t chash_size;
+    uint32_t *cstart; uint32_t cstart_size;   // direct cell table: first sorted index per cell of the occupied box (k_bp_cell_starts)
     uint32_t *large_list;
     uint32_t *newcount, *newoff;
     uint2 *newpairs;
