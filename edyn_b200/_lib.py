@@ -54,7 +54,7 @@ class Stats(C.Structure):
 EXPORTS = ["b2d_create", "b2d_destroy", "b2d_last_error", "b2d_add_bodies", "b2d_remove_bodies", "b2d_wake_bodies", "b2d_download_sleeping", "b2d_add_hinges", "b2d_add_exclusions", "b2d_remove_exclusions",
            "b2d_step", "b2d_run_phases", "b2d_upload_state", "b2d_download_state", "b2d_num_manifolds",
            "b2d_download_pairs", "b2d_download_contacts", "b2d_upload_contacts", "b2d_download_islands",
-           "b2d_download_solver_order", "b2d_download_hinge_impulses", "b2d_get_stats", "b2d_reset_timers", "b2d_debug_counters", "b2d_debug_tiles", "b2d_debug_tile_map", "b2d_device_bounds", "b2d_set_halo_margin", "b2d_sync", "b2d_stream",
+           "b2d_download_solver_order", "b2d_download_hinge_impulses", "b2d_get_stats", "b2d_reset_timers", "b2d_debug_counters", "b2d_debug_tiles", "b2d_debug_newcount", "b2d_debug_tile_map", "b2d_device_bounds", "b2d_set_halo_margin", "b2d_sync", "b2d_stream",
            "b2d_upload_bodies", "b2d_set_entities", "b2d_download_entities", "b2d_island_halo", "b2d_handover_plan",
            "b2d_handover_bytes", "b2d_handover_pack", "b2d_handover_unpack", "b2d_set_timing", "b2d_raycast", "b2d_raycast_device",
            "b2d_set_material_mixing", "b2d_remove_material_mixing", "b2d_update_presentation", "b2d_snap_presentation",

@@ -32,6 +32,7 @@ struct b2d_world {
     int tile_fused_blocks = 0, tile_fused_blocks_2p = 0;     // grids of the island-tile kernels (CTAs loop over the tiles)
     int cell_key_bits = 48;                         // sum of d.cell_bits: end bit of the cell sort
     uint32_t bp_warp_max = 100000;                  // neighbourhood search: warp per body up to this many bodies (B2D_BP_WARP_MAX)
+    bool bp_half = true;                            // thread-per-body count pass over half the neighbourhood (B2D_BP_HALF=0: the whole)
     void *cub_tmp = nullptr; size_t cub_tmp_bytes = 0;
     float *stage = nullptr; size_t stage_floats = 0;        // device staging for packed host arrays
     uint64_t launches = 0, steps = 0;
@@ -182,7 +183,8 @@ b2d_world *b2d_create(const b2d_config *cfg) {
     if (const char *e = getenv("B2D_BP_CELL_TABLE")) cells_per_body = (uint64_t)std::max(0, atoi(e));
     d.cstart_size = (uint32_t)std::min<uint64_t>(cells_per_body * NB, 0xFFFFFFFFull);
     ok = ok && dalloc(w, d.cstart, d.cstart_size, 0xFF);
-    ok = ok && dalloc(w, d.large_list, NB) && dalloc(w, d.newcount, NB) && dalloc(w, d.newoff, NB) && dalloc(w, d.newpairs, NM);
+    if (const char *e = getenv("B2D_BP_HALF")) w->bp_half = atoi(e) != 0;
+    ok = ok && dalloc(w, d.large_list, NB) && dalloc(w, d.lmask, NB) && dalloc(w, d.newcount, NB) && dalloc(w, d.newoff, NB) && dalloc(w, d.newpairs, NM);
     ok = ok && dalloc(w, d.free_flag, NM) && dalloc(w, d.free_rank, NM) && dalloc(w, d.free_list, NM);
     d.mhash_size = pow2_at_least(2ull * NM);
     ok = ok && dalloc(w, d.mhash_key, d.mhash_size, 0xFF) && dalloc(w, d.mhash_val, d.mhash_size);
@@ -634,21 +636,24 @@ int b2d_remove_material_mixing(b2d_world *w, uint32_t n, const uint32_t *id0, co
 
 static int enqueue_broadphase(b2d_world *w) {
     Dev &d = w->d; cudaStream_t s = w->stream;
+    if (d.nbodies) {        // first: k_bp_cells also zeroes lmask, which k_bp_separate fills, and newcount
+        CK(cudaMemsetAsync(d.cell_box, 0xFF, 6 * sizeof(uint32_t), s));
+        LAUNCH(k_bp_cells, d.nbodies, 256, d, d.cellkey, d.cellbody, d.cell_box);
+    }
     CK(cudaMemsetAsync(d.mhash_key, 0xFF, (size_t)d.mhash_size * sizeof(unsigned long long), s));
     LAUNCH(k_bp_separate, d.NM, 256, d);
     size_t t = w->cub_tmp_bytes;
     CK(cub::DeviceScan::ExclusiveSum(w->cub_tmp, t, d.free_flag, d.free_rank, (int)d.NM, s)); ++w->launches;
     LAUNCH(k_bp_free_list, d.NM, 256, d);
     if (d.nbodies) {
-        CK(cudaMemsetAsync(d.cell_box, 0xFF, 6 * sizeof(uint32_t), s));
-        LAUNCH(k_bp_cells, d.nbodies, 256, d, d.cellkey, d.cellbody, d.cell_box);
         LAUNCH(k_bp_cell_mode, d.chash_size, 256, d);            // direct table or cell hash (clears the hash when it is used)
         t = w->cub_tmp_bytes;
         CK(cub::DeviceRadixSort::SortPairs(w->cub_tmp, t, d.cellkey, d.cellkey_s, d.cellbody, d.cellbody_s, (int)d.nbodies, 0, w->cell_key_bits, s)); w->launches += 4;
         LAUNCH(k_bp_cell_starts, d.nbodies, 256, d);
         // a warp per query body while that still fills the machine with few bodies, a thread per body beyond
         const bool bp_warp = d.nbodies <= w->bp_warp_max;
-        if (bp_warp) LAUNCH(k_bp_pairs_warp<false>, (uint64_t)d.nbodies * 32, 256, d); else LAUNCH(k_bp_pairs<false>, d.nbodies, 128, d);
+        void (*count_pass)(Dev) = w->bp_half ? k_bp_pairs<false, true> : k_bp_pairs<false, false>;
+        if (bp_warp) LAUNCH(k_bp_pairs_warp<false>, (uint64_t)d.nbodies * 32, 256, d); else LAUNCH(count_pass, d.nbodies, 128, d);
         t = w->cub_tmp_bytes;
         CK(cub::DeviceScan::ExclusiveSum(w->cub_tmp, t, d.newcount, d.newoff, (int)d.nbodies, s)); ++w->launches;
         if (bp_warp) LAUNCH(k_bp_pairs_warp<true>, (uint64_t)d.nbodies * 32, 256, d); else LAUNCH(k_bp_pairs<true>, d.nbodies, 128, d);
@@ -1242,6 +1247,14 @@ int b2d_debug_counters(b2d_world *w, void *out, uint32_t bytes) {
     cudaSetDevice(w->cfg.device);
     CK(cudaStreamSynchronize(w->stream));
     CK(cudaMemcpy(out, w->d.cnt, std::min<size_t>(bytes, sizeof(Counters)), cudaMemcpyDeviceToHost));
+    return B2D_OK;
+}
+// development aid: the last broadphase's newcount
+int b2d_debug_newcount(b2d_world *w, uint32_t *counts) {
+    if (!w || !counts) return B2D_ERR_ARGUMENT;
+    cudaSetDevice(w->cfg.device);
+    CK(cudaStreamSynchronize(w->stream));
+    if (w->d.nbodies) CK(cudaMemcpy(counts, w->d.newcount, w->d.nbodies * sizeof(uint32_t), cudaMemcpyDeviceToHost));
     return B2D_OK;
 }
 // development aid: island tiles of the last step: out = {tiles, tiled manifolds, tiled hinges, manifolds with rows, hinges with rows, max bodies per tile}

@@ -190,6 +190,16 @@ __global__ void k_remove_hinges(Dev d) {
         if (ra || rb) { const uint32_t dead = ra ? p.x : p.y; d.hpair[h] = make_uint2(dead, dead); d.hcolor[h] = COLOR_NONE; }
     }
 }
+// A surviving manifold with a large side: the bit of that body's large_list index (below 32) in the other body's lmask,
+// so the count pass knows the pair exists without probing mhash.  nlarge is small: a scan finds the index.
+B2D_D void bp_mark_large(const Dev &d, uint2 p, uint32_t fx, uint32_t fy) {
+    const uint32_t n = min(d.nlarge, 32u);
+    for (uint32_t k = 0; k < n; ++k) {
+        const uint32_t l = d.large_list[k];
+        if ((fy & F_LARGE) && l == p.y) atomicOr(&d.lmask[p.x], 1u << k);
+        if ((fx & F_LARGE) && l == p.x) atomicOr(&d.lmask[p.y], 1u << k);
+    }
+}
 __global__ void k_bp_separate(Dev d) {
     const uint32_t hwm = d.cnt->hwm;
     GRID_STRIDE(m, d.NM) {
@@ -198,13 +208,15 @@ __global__ void k_bp_separate(Dev d) {
             uint32_t st = d.mstate[m];
             if (st & MS_ALIVE) {
                 uint2 p = d.mpair[m];
+                const uint32_t fx = d.flags[p.x], fy = d.flags[p.y];
                 // a destroyed body takes its graph edges with it (island_manager.cpp:47-66)
-                if (((d.flags[p.x] | d.flags[p.y]) & F_REMOVED) || !intersect(inset(body_box(d, p.x), BP_SEPARATION), body_box(d, p.y))) {
+                if (((fx | fy) & F_REMOVED) || !intersect(inset(body_box(d, p.x), BP_SEPARATION), body_box(d, p.y))) {
                     d.mstate[m] = COLOR_NONE << MS_COLOR_SHIFT;      // clear_contact_manifold + destroy
                     d.cnt->graph_changed = 1u;
                     flag = 1;
                 } else {
                     hash_insert(d.mhash_key, d.mhash_val, d.mhash_size, pair_key(p.x, p.y), m);
+                    if ((fx | fy) & F_LARGE) bp_mark_large(d, p, fx, fy);
                 }
             } else flag = 1;
         }
@@ -276,10 +288,12 @@ B2D_D void cell_of(const Dev &d, uint32_t i, int &cx, int &cy, int &cz) { cell_o
 
 // Cell key per body.  Shapeless and "large" bodies get the all-ones key and sort to the end.  The broadphase writes
 // d.cellkey / d.cellbody and the occupied box of key fields (box: min field, then min of the complemented field, both
-// preset to all-ones); the raycast index (k_ray_*) its own arrays and no box.
+// preset to all-ones), and zeroes the per-body accumulators of its step (lmask for k_bp_separate, newcount for the
+// count pass); the raycast index (k_ray_*) writes its own arrays and no box.
 __global__ void k_bp_cells(Dev d, unsigned long long *cellkey, uint32_t *cellbody, uint32_t *box) {
     uint32_t m[6] = {~0u, ~0u, ~0u, ~0u, ~0u, ~0u};
     GRID_STRIDE(i, d.nbodies) {
+        if (box) { d.lmask[i] = 0u; d.newcount[i] = 0u; }
         uint32_t f = d.flags[i];
         unsigned long long key = EMPTY_KEY;
         if (shape_of(f) != SH_NONE && !(f & F_LARGE)) {
@@ -430,22 +444,64 @@ B2D_D BpColumn bp_column_find(const Dev &d, const CellBox &box, bool direct, int
     }
     return c;
 }
-B2D_D void bp_column_walk(const Dev &d, const BpColumn &c, uint32_t A, uint32_t fA, const box3 &bbA, const box3 &qA,
-                          uint32_t &count, uint2 *out) {
+// visit(k) for every sorted record k of the column's cells, in key order.
+template<typename Visit>
+B2D_D void bp_column_walk(const Dev &d, const BpColumn &c, Visit visit) {
     bool found = false; uint32_t k = 0;
     #pragma unroll
     for (int z = 0; z < 3; ++z) {
         if (!found && c.occ[z]) { found = true; k = c.start[z]; }
         if (z == 2 || c.key[z + 1] != c.key[z] + 1) {             // the run ends at cell z
-            if (found) for (; k < d.nbodies && d.cellkey_s[k] <= c.key[z]; ++k) bp_candidate_rec(d, A, fA, bbA, qA, k, count, out);
+            if (found) for (; k < d.nbodies && d.cellkey_s[k] <= c.key[z]; ++k) visit(k);
             found = false;
         }
     }
 }
 
-template<bool FILL>
+// Count pass over half the neighbourhood: each pair of grid bodies is met once, by the one earlier in the cell order.
+// The pair is evaluated by bp_candidate from the side the whole-neighbourhood walk takes it (the higher-id dynamic
+// body, or the dynamic one), on the same arguments, so the decision is the same.  When that query body is the other
+// record, its count goes up by an atomicAdd: only for a new pair, rare once a scene has settled.
+B2D_D void bp_half_candidate(const Dev &d, uint32_t A, uint32_t fA, const box3 &bbA, uint32_t k, uint32_t &count) {
+    const float4 mn = d.bprec_min[k], mx = d.bprec_max[k];
+    const uint32_t j = __float_as_uint(mn.w), fj = __float_as_uint(mx.w);
+    const bool dA = is_dynamic(fA), dj = is_dynamic(fj);
+    if (!dA && !dj) return;
+    const bool mine = dA && (!dj || A > j);             // A is the query body
+    const box3 bbj = rec_box(mn, mx);
+    const box3 bq = mine ? bbA : bbj, bc = mine ? bbj : bbA;
+    uint32_t c = 0;
+    bp_candidate(d, mine ? A : j, mine ? fA : fj, bq, inset(bq, BP_OFFSET), mine ? j : A, mine ? fj : fA, bc, c, nullptr);
+    if (c) { if (mine) ++count; else atomicAdd(&d.newcount[j], 1u); }
+}
+// The records after t in the 27 cells around it: the later records of its own cell and the cells with greater keys (x is
+// the key's high field, z the low one).  Those of its own column follow t directly and need no lookup; columns whose
+// keys are all below its own (x - 1, and y - 1 at its own x) are skipped; clamped offsets are deduplicated as in the
+// whole walk.  Two bodies whose AABBs can meet have centres less than a cell apart, so each lies in the other's
+// neighbourhood, clamped or not, and the pairs met are those of the whole walk.
+B2D_D void bp_half_walk(const Dev &d, uint32_t t, uint32_t A, uint32_t fA, const box3 &bbA, int cx, int cy, int cz, uint32_t &count) {
+    auto visit = [&](uint32_t k) { bp_half_candidate(d, A, fA, bbA, k, count); };
+    const unsigned long long last = cell_key_of(d, cx, cy, cz + 1);
+    for (uint32_t k = t + 1; k < d.nbodies && d.cellkey_s[k] <= last; ++k) visit(k);
+    const CellBox box = load_cell_box(d);
+    const bool direct = d.cnt->bp_direct;
+    for (int dx = 0; dx <= 1; ++dx) {
+        if (dx > 0 && cell_field(d, 0, cx + 1) == cell_field(d, 0, cx)) continue;      // clamped: its own x
+        for (int dy = dx > 0 ? -1 : 1; dy <= 1; ++dy) {
+            if (dy > -1 && cell_field(d, 1, cy + dy) == cell_field(d, 1, cy + dy - 1)) continue;
+            bp_column_walk(d, bp_column_find(d, box, direct, cx + dx, cy + dy, cz), visit);
+        }
+    }
+}
+
+// HALF: the count pass over half the neighbourhood (bp_half_walk) with the large list screened by lmask; every grid
+// body walks, whatever its kind.  Otherwise each dynamic body walks the whole neighbourhood (the fill pass, and the count
+// pass with B2D_BP_HALF=0).
+template<bool FILL, bool HALF = false>
 // (launch bounds: at most 56 registers, nine CTAs of 128 per SM, the residency the search had before the direct table)
 __global__ void __launch_bounds__(128, 9) k_bp_pairs(Dev d) {
+    static_assert(!(FILL && HALF), "the fill pass writes each query body's pairs in the order of the whole walk");
+    if (!FILL && blockIdx.x == 0 && threadIdx.x == 0) d.cnt->bp_count_walk = HALF ? 2u : 1u;
     GRID_STRIDE(t, d.nbodies) {
         // threads walk the bodies in cell order: a warp's queries hit the same cells and candidate records (output
         // slots are still indexed by body id, so the pair order does not change)
@@ -460,26 +516,42 @@ __global__ void __launch_bounds__(128, 9) k_bp_pairs(Dev d) {
             if ((unsigned long long)d.newoff[A] + d.newcount[A] > d.NM) { atomicOr(&d.cnt->err, ERR_MANIFOLD_CAPACITY); continue; }
             out = d.newpairs + d.newoff[A];
         }
-        if (is_dynamic(fA) && shape_of(fA) != SH_NONE) {
+        const bool shaped = shape_of(fA) != SH_NONE;
+        const bool query = is_dynamic(fA) && shaped;
+        if (HALF ? shaped : query) {
             const box3 bbA = rec_box(rmn, rmx);
             const box3 qA = inset(bbA, BP_OFFSET);
             if (!(fA & F_LARGE)) {
                 int cx, cy, cz; cell_of(d, rmn, rmx, cx, cy, cz);
-                const CellBox box = load_cell_box(d);
-                const bool direct = d.cnt->bp_direct;
-                for (int dx = -1; dx <= 1; ++dx) {
-                    if (dx > -1 && cell_field(d, 0, cx + dx) == cell_field(d, 0, cx + dx - 1)) continue;      // clamped: same cells
-                    for (int dy = -1; dy <= 1; ++dy) {
-                        if (dy > -1 && cell_field(d, 1, cy + dy) == cell_field(d, 1, cy + dy - 1)) continue;
-                        bp_column_walk(d, bp_column_find(d, box, direct, cx + dx, cy + dy, cz), A, fA, bbA, qA, count, out);
+                if (HALF) {
+                    bp_half_walk(d, t, A, fA, bbA, cx, cy, cz, count);
+                } else {
+                    const CellBox box = load_cell_box(d);
+                    const bool direct = d.cnt->bp_direct;
+                    for (int dx = -1; dx <= 1; ++dx) {
+                        if (dx > -1 && cell_field(d, 0, cx + dx) == cell_field(d, 0, cx + dx - 1)) continue;      // clamped: same cells
+                        for (int dy = -1; dy <= 1; ++dy) {
+                            if (dy > -1 && cell_field(d, 1, cy + dy) == cell_field(d, 1, cy + dy - 1)) continue;
+                            bp_column_walk(d, bp_column_find(d, box, direct, cx + dx, cy + dy, cz),
+                                           [&](uint32_t k) { bp_candidate_rec(d, A, fA, bbA, qA, k, count, out); });
+                        }
                     }
                 }
-            } else {
+            } else if (query) {
                 for (uint32_t j = 0; j < d.nbodies; ++j) if (!(d.flags[j] & F_LARGE)) bp_candidate_id(d, A, fA, bbA, qA, j, count, out);
             }
-            for (uint32_t k = 0; k < d.nlarge; ++k) bp_candidate_id(d, A, fA, bbA, qA, d.large_list[k], count, out);
+            if (query) {
+                // HALF: a set bit of lmask is a manifold alive with that large body, so the pair cannot be new (large
+                // query bodies included: bp_mark_large sets the bit on both sides of a manifold between two large bodies)
+                const uint32_t known = HALF ? d.lmask[A] : 0u;
+                for (uint32_t k = 0; k < d.nlarge; ++k)
+                    if (k >= 32 || !((known >> k) & 1u)) bp_candidate_id(d, A, fA, bbA, qA, d.large_list[k], count, out);
+            }
         }
-        if (!FILL) d.newcount[A] = count;
+        if (!FILL) {
+            if (!HALF) d.newcount[A] = count;
+            else if (count) atomicAdd(&d.newcount[A], count);      // other threads may count pairs of A as well
+        }
     }
 }
 // The same search with one WARP per query body: lane c < 27 takes cell c of the neighbourhood (in the loop order of

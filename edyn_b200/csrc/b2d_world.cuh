@@ -90,6 +90,7 @@ struct Counters {
     unsigned long long steps_rebuilt, steps_reused;          // graph steps that ran / skipped the rebuild (statistics)
     unsigned long long dbg[16];  // development counters (B2D_DF_PROFILE builds only)
     uint32_t bp_direct;          // this step's cell lookup: 1 the direct table (Dev::cstart), 0 the cell hash (k_bp_cell_mode)
+    uint32_t bp_count_walk;      // the last thread-per-body count pass: 1 the whole neighbourhood, 2 half of it (k_bp_pairs)
 };
 
 struct Dev {
@@ -131,6 +132,7 @@ struct Dev {
     unsigned long long *chash_key; uint32_t *chash_val; uint32_t chash_size;
     uint32_t *cstart; uint32_t cstart_size;   // direct cell table: first sorted index per cell of the occupied box (k_bp_cell_starts)
     uint32_t *large_list;
+    uint32_t *lmask;                     // per body: bit k set while an alive manifold joins it to large_list[k], k < 32 (k_bp_separate)
     uint32_t *newcount, *newoff;
     uint2 *newpairs;
     uint32_t *free_flag, *free_rank, *free_list;

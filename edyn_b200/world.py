@@ -389,6 +389,12 @@ class World:
         self._check(self.l.b2d_debug_tiles(self.h, _p(out)))
         return dict(zip(("tiles", "tiled_manifolds", "tiled_hinges", "active_manifolds", "active_hinges", "max_bodies_per_tile"), out.tolist()))
 
+    def debug_newcount(self):
+        """Development aid: the new pairs the last broadphase counted per body (b2d_debug_newcount)."""
+        out = np.zeros(max(1, self.num_bodies), np.uint32)
+        self._check(self.l.b2d_debug_newcount(self.h, _p(out)))
+        return out[:self.num_bodies]
+
     def debug_tile_map(self):
         """Development aid: the island-tile packing of the last rebuild (b2d_debug_tile_map).  Per body its tile and record
         slot (0xFFFFFFFF / 0xFFFF: not tiled); per tile its body count and its [c0, c1) / [h0, h1) ranges into

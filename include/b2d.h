@@ -231,6 +231,8 @@ int b2d_debug_counters(b2d_world *w, void *out, uint32_t bytes);
 /* Development aid: the island tiles of the last step (DESIGN.md section 2): out6 = tiles, manifolds / hinges solved in
  * tiles, manifolds / hinges with rows, most bodies in one tile. */
 int b2d_debug_tiles(b2d_world *w, uint32_t *out6);
+/* Development aid: the new pairs the last broadphase counted per body (each pair at its query body), one word per body. */
+int b2d_debug_newcount(b2d_world *w, uint32_t *counts);
 /* Development aid: the island-tile packing of the last island rebuild, which later steps reuse while the constraint graph
  * is unchanged.  counts5 = tiles (two-point tiles first), two-point tiles, manifolds / hinges solved in tiles, tile
  * capacity of the world.  Each of the other outputs may be NULL: btile / bslot (one word per body: its tile and record
